@@ -1,4 +1,4 @@
-/* nksr_b200 -- C-ABI of the B200-native NKSR reconstruction hot path.
+/* nksr_b200 -- C-ABI of the H100-native (sm_90a) NKSR reconstruction hot path.
  *
  * Every entry point is `extern "C"`, takes plain device pointers + sizes + a cudaStream_t
  * (passed as void*), performs NO allocation (the caller owns every buffer, normally torch
@@ -6,7 +6,7 @@
  * a *_count / capacity call, the caller allocates, a *_fill call.
  *
  * The reference ships this path as the closed `nksr` wheel, so each group below cites the
- * reference CALL SITE whose behaviour it replaces (paths relative to /root/reference).
+ * reference CALL SITE whose behaviour it replaces (paths relative to the reference checkout, nv-tlabs/NKSR @ 0d4e369).
  * The reference-side binding is the ctypes shim in nksr_b200/_lib.py (see INTEGRATION.md).
  */
 #ifndef NKSR_B200_H
@@ -103,8 +103,8 @@ NKSR_API int nksr_pool_children(const int32_t* child8, const float* in, int64_t 
  * idx = nbr27[l] (K = 27): 3x3x3 convolution on level l; idx = child8[l+1] (K = 8): stride-2 convolution l -> l+1.
  * c_in and c_out multiples of 32; bias / res may be NULL; relu: 0/1; tf32: 0 = fp32 FFMA, 1 = mma.sync TF32 (fp32
  * accumulation, operands rounded to TF32 in the kernel, K <= 32), 2 = the same with W already rounded to TF32 by the
- * caller (low 13 mantissa bits zero), 3 = tcgen05.mma kind::tf32 with the accumulator in TMEM (K <= 32 x 32-channel
- * steps staged in SWIZZLE_128B shared memory by cp.async; W rounded to TF32 by the caller AND transposed to
+ * caller (low 13 mantissa bits zero), 3 = wgmma.mma_async tf32 with the accumulator in registers (K <= 32 x 32-channel
+ * steps staged in 128-byte-swizzled shared memory by cp.async; W rounded to TF32 by the caller AND transposed to
  * K x c_out x c_in, the tensor core's K-major operand order) */
 NKSR_API int nksr_gather_gemm(const float* x, const int32_t* idx, int64_t n_out, int K, const float* W,
                      const float* bias, const float* res, float* y, int c_in, int c_out, int relu, int tf32,

@@ -1,4 +1,4 @@
-"""Drop-in alias: `import nksr` resolves to the B200-native implementation (nksr_b200), so the
+"""Drop-in alias: `import nksr` resolves to the H100-native implementation (nksr_b200), so the
 reference's examples/*.py and models/nksr_net.py import unchanged (SURVEY.md Appendix A)."""
 import sys as _sys
 

@@ -1,9 +1,9 @@
-"""nksr_b200 -- B200-native implementation of the NKSR reconstruction hot path.
+"""nksr_b200 -- H100-native implementation of the NKSR reconstruction hot path.
 
 Same Python surface as the reference's closed `nksr` wheel (SURVEY.md Appendix A):
 Reconstructor, SparseFeatureHierarchy, NKSRNetwork, fields.{KernelField, NeuralField,
 LayerField, PCNNField}, configs.load_checkpoint_from_url, get_estimate_normal_preprocess_fn.
-All arithmetic of the hot path runs in hand-written sm_100a CUDA kernels behind the C-ABI of
+All arithmetic of the hot path runs in hand-written sm_90a CUDA kernels behind the C-ABI of
 include/nksr_b200.h (nksr_b200/libnksr_b200.so); there is no CPU or PyTorch fallback.
 Inference only: the solve is not differentiable (the reference needs that for training only).
 """

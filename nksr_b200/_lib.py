@@ -195,7 +195,7 @@ def call(name: str, *args):
 
 def require_cuda(t: torch.Tensor, what: str):
     if not t.is_cuda:
-        raise NksrError(f"{what} must live on a CUDA device: nksr_b200 is a B200-only implementation "
+        raise NksrError(f"{what} must live on a CUDA device: nksr_b200 is a CUDA-only implementation "
                         "(no CPU path; the CPU oracle under oracle/ is test infrastructure)")
 
 

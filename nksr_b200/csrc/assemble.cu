@@ -13,10 +13,10 @@
 // such row r contributes  w * E[r,i] * E[r, :]  and all rows of u share the same 27-stencils on
 // level l and on every coarser level, so lane s accumulates stencil slot s in a register and
 // the warp flushes once per u into a per-warp shared-memory tile indexed by structural slot --
-// no atomics, deterministic summation order.  The round-1 ncu captures (profiles/r1a..r1d) showed the
+// no atomics, deterministic summation order.  Profiles of the first version showed the
 // kernel to be instruction-issue / L2-latency bound, hence: neighbour indices and row ranges are
 // fetched lane-parallel once per row; constraint rows are stored location-major so every line is a
-// compile-time offset from one pointer; two levels are accumulated per packed FFMA2; 64 registers keep
+// compile-time offset from one pointer; two levels are accumulated per float2 pair of FMAs; 64 registers keep
 // 32 warps per SM resident; and on the coarse levels (a voxel owns hundreds of constraint rows) the
 // 27 x 27 products are reduced once per voxel by k_gram_blocks and the rows only gather block lines.
 // Optional compact gradient rows (approx_kernel_grad: one line <phi,z_s> + tau per location and level,
@@ -88,7 +88,7 @@ k_place_rank(nksr_svh_t svh, int l, int k, int32_t* __restrict__ rank8, int32_t*
   int64_t first, end;
   if (k == 1 && svh.child8[lu] != nullptr) {
     // children are contiguous in Morton order: one 32-byte row of the child table instead of two binary searches
-    // over the level's keys (r2e: 8.1 ms of the 14.3 ms of the six rank kernels were the (0,1) pair's searches)
+    // over the level's keys (the searches were most of the rank kernels' time)
     const int c = lane < 8 ? __ldg(svh.child8[lu] + a * 8 + lane) : -1;
     int lo = c >= 0 ? c : 0x7fffffff, hi = c;
 #pragma unroll
@@ -177,16 +177,16 @@ k_place_prefix(nksr_svh_t svh, int l, int k, const int32_t* __restrict__ class_c
 // ONCE, instead of each of the 27 matrix rows around u streaming all of u's constraint rows again.
 // Block layout: 28 lines of 32 floats -- lines 0..26 = M[si][:], line 27 = rhs share per si (k = 0).
 // m[s] += el[s] * ek for the 27 stencil slots s (lane = column of the block, m[s] = row s): the weighted level-l line
-// `el` of the constraint row is staged in shared memory and read back as seven broadcast 128-bit loads feeding 14 packed
-// FFMA2 (sm_100) -- the first version fetched the 28 values with 28 shuffles per row, two thirds of its instructions
+// `el` of the constraint row is staged in shared memory and read back as seven broadcast 128-bit loads feeding 14
+// float2 FMA pairs -- the first version fetched the 28 values with 28 shuffles per row, two thirds of its instructions
 __device__ __forceinline__ void gram_block_update(float (&m)[28], const float* __restrict__ el_line, float ek) {
   const float2 ek2 = make_float2(ek, ek);
   const float4* l4 = reinterpret_cast<const float4*>(el_line);
 #pragma unroll
   for (int j = 0; j < 7; ++j) {
     const float4 a = l4[j];                                    // slot 27 is padding (zero)
-    const float2 r0 = __ffma2_rn(make_float2(a.x, a.y), ek2, make_float2(m[4 * j], m[4 * j + 1]));
-    const float2 r1 = __ffma2_rn(make_float2(a.z, a.w), ek2, make_float2(m[4 * j + 2], m[4 * j + 3]));
+    const float2 r0 = ffma2_rn(make_float2(a.x, a.y), ek2, make_float2(m[4 * j], m[4 * j + 1]));
+    const float2 r1 = ffma2_rn(make_float2(a.z, a.w), ek2, make_float2(m[4 * j + 2], m[4 * j + 3]));
     m[4 * j] = r0.x; m[4 * j + 1] = r0.y; m[4 * j + 2] = r1.x; m[4 * j + 3] = r1.y;
   }
 }
@@ -238,7 +238,7 @@ k_gram_blocks(nksr_svh_t svh, nksr_constraints_t cs, float* __restrict__ mblocks
   if (cs.range_nrm) {
     const int32_t* rn = cs.range_nrm + 2 * (svh.offset[l] + u);
     const int nb = __ldg(rn), ne = __ldg(rn + 1);
-    // (requesting the lines of location q + 1 before location q is multiplied in was tried: 33.4 ms instead of 22.8, r2t)
+    // (requesting the lines of location q + 1 before location q is multiplied in was tried: slower)
     for (int q = nb; q < ne; ++q) {
       const float* p0 = cs.e_nrm + ((int64_t)q * L + l) * (3 * NKSR_ROW_STRIDE) + lane;
       float ek[3];
@@ -271,7 +271,7 @@ k_gram_blocks(nksr_svh_t svh, nksr_constraints_t cs, float* __restrict__ mblocks
 
 // ILV (MAXL == 4): rows in the interleaved layout -- one 128-bit load per lane brings the four levels of a location
 // (value rows) or of one axis of it (gradient rows): 1 + 3 wide loads per visited location instead of 4 + 12 narrow ones
-// (r2f: 13.6 G load requests, the LSU the busiest unit of the kernel).  Same products in the same order: the matrix is
+// (with narrow loads the LSU was the busiest unit of the kernel).  Same products in the same order: the matrix is
 // bitwise the one of the plain layout.
 template <bool COMPACT, int MAXL, int MINB, bool PLACED, bool ILV>
 __global__ void __launch_bounds__(kWarps * 32, MINB)
@@ -363,8 +363,8 @@ k_gram_fill(nksr_svh_t svh, nksr_feat_t feat, nksr_constraints_t cs, int64_t n_t
       for (int q = pb; q < pe; ++q) {
         const float4 v = __ldg(ep + (int64_t)q * NKSR_ROW_STRIDE);
         const float a = cs.w_pos * __shfl_sync(0xffffffffu, level_of(v, l), si);
-        a01 = __ffma2_rn(make_float2(a, a), make_float2(v.x, v.y), a01);
-        a23 = __ffma2_rn(make_float2(a, a), make_float2(v.z, v.w), a23);
+        a01 = ffma2_rn(make_float2(a, a), make_float2(v.x, v.y), a01);
+        a23 = ffma2_rn(make_float2(a, a), make_float2(v.z, v.w), a23);
       }
       const float4* en = reinterpret_cast<const float4*>(cs.e_nrm) + lane;
       for (int q = nb; q < ne; ++q) {
@@ -377,8 +377,8 @@ k_gram_fill(nksr_svh_t svh, nksr_feat_t feat, nksr_constraints_t cs, int64_t n_t
           const float a = cs.w_nrm * __ldg(ps + ax * (4 * NKSR_ROW_STRIDE));
           bsum = fmaf(a, __ldg(t + ax), bsum);
           const float4 v = __ldg(p + ax * NKSR_ROW_STRIDE);
-          a01 = __ffma2_rn(make_float2(a, a), make_float2(v.x, v.y), a01);
-          a23 = __ffma2_rn(make_float2(a, a), make_float2(v.z, v.w), a23);
+          a01 = ffma2_rn(make_float2(a, a), make_float2(v.x, v.y), a01);
+          a23 = ffma2_rn(make_float2(a, a), make_float2(v.z, v.w), a23);
         }
       }
       // absolute -> relative levels (l is uniform in the warp)
@@ -387,7 +387,7 @@ k_gram_fill(nksr_svh_t svh, nksr_feat_t feat, nksr_constraints_t cs, int64_t n_t
       else if (l == 2) { r[0] = a23.x; r[1] = a23.y; }
       else { r[0] = a23.y; }
     } else {
-    // packed fp32 FMAs (FFMA2, sm_100): two levels per instruction, same IEEE result per lane
+    // fp32 FMAs on float2 pairs: two levels per step, same IEEE result per lane
     float2 r2[MAXL / 2];
 #pragma unroll
     for (int k2 = 0; k2 < MAXL / 2; ++k2) r2[k2] = make_float2(0.f, 0.f);
@@ -399,7 +399,7 @@ k_gram_fill(nksr_svh_t svh, nksr_feat_t feat, nksr_constraints_t cs, int64_t n_t
       const float a = cs.w_pos * __shfl_sync(0xffffffffu, ln[0], si);
 #pragma unroll
       for (int k2 = 0; k2 < MAXL / 2; ++k2)
-        r2[k2] = __ffma2_rn(make_float2(a, a), make_float2(ln[2 * k2], ln[2 * k2 + 1]), r2[k2]);
+        r2[k2] = ffma2_rn(make_float2(a, a), make_float2(ln[2 * k2], ln[2 * k2 + 1]), r2[k2]);
     }
     if (COMPACT) {
       // one line per (location, level): <phi,z_s> in slots 0..26, tau in 27..29;
@@ -433,12 +433,12 @@ k_gram_fill(nksr_svh_t svh, nksr_feat_t feat, nksr_constraints_t cs, int64_t n_t
       }
     } else {
       // (a "wide" variant -- 80 registers, three blocks per SM, two normal locations = 30 line loads in flight per warp
-      // -- was measured at 187 ms against 175 ms, r2l, and removed)
+      // -- was measured slower and removed)
       for (int q = nb; q < ne; ++q) {
         const float* p0 = cs.e_nrm + ((int64_t)q * L + l) * (3 * NKSR_ROW_STRIDE);
         const float* t = cs.t_nrm + (int64_t)q * 3;
         // (the own coefficient stays a broadcast LOAD here: fetching it by shuffle from the level-l line -- as the position
-        // loop does -- ties the three axes' loads to the shuffles' completion and cost 42 ms on cfg4, r2g)
+        // loop does -- ties the three axes' loads to the shuffles' completion and was measured slower)
 #pragma unroll
         for (int ax = 0; ax < 3; ++ax) {
           const float a = cs.w_nrm * __ldg(p0 + ax * NKSR_ROW_STRIDE + si);
@@ -448,7 +448,7 @@ k_gram_fill(nksr_svh_t svh, nksr_feat_t feat, nksr_constraints_t cs, int64_t n_t
           for (int k2 = 0; k2 < MAXL / 2; ++k2) {
             const float l0 = 2 * k2 <= nup ? __ldg(pk + (2 * k2) * nrm_level) : 0.f;
             const float l1 = 2 * k2 + 1 <= nup ? __ldg(pk + (2 * k2 + 1) * nrm_level) : 0.f;
-            r2[k2] = __ffma2_rn(make_float2(a, a), make_float2(l0, l1), r2[k2]);
+            r2[k2] = ffma2_rn(make_float2(a, a), make_float2(l0, l1), r2[k2]);
           }
         }
       }
@@ -458,8 +458,8 @@ k_gram_fill(nksr_svh_t svh, nksr_feat_t feat, nksr_constraints_t cs, int64_t n_t
     }  // !ILV
     }  // !use_blocks
     // flush: every lane < 27 owns a distinct structural slot per level; slot = base of the source voxel (computed once
-    // per row by lane `us`, see flush_base above) + constant of the lane.  (r2b source page: the per-lane index
-    // arithmetic of the first version was 36 + 3 x 18 instructions 17 times per row, 21 % of the kernel.)
+    // per row by lane `us`, see flush_base above) + constant of the lane.  (The per-lane index arithmetic
+    // of the first version was a fifth of the kernel's instructions.)
     {
       const unsigned wa = __shfl_sync(0xffffffffu, flush_a, us), wb = __shfl_sync(0xffffffffu, flush_b, us);
       if (lane < 27) {
@@ -494,8 +494,7 @@ k_gram_fill(nksr_svh_t svh, nksr_feat_t feat, nksr_constraints_t cs, int64_t n_t
   __syncwarp();
   // write-out in structural order: the 125 same-level slots (4 chunks of 32), then the 64 slots of every coarser level
   // (2 chunks each) -- the level offset k is uniform inside a chunk, so the box bounds, the ancestor and its parent are
-  // computed once per level instead of once per slot (r2b source page: 86 + 31 instructions per chunk of slot
-  // arithmetic in the first version, where a chunk could straddle two levels)
+  // computed once per level instead of once per slot (in the first version a chunk could straddle two levels)
   const int64_t p0 = rowptr[row];
   int written = 0;
   auto emit = [&](const int c, const int k, const int t, const int ds, const int sm) {

@@ -1,4 +1,4 @@
-// Shared device helpers for the nksr_b200 kernels (sm_100a).
+// Shared device helpers for the nksr_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -83,6 +83,11 @@ __device__ __forceinline__ double warp_sum_d(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
+}
+
+// c + a * b on a pair of fp32 values, each an IEEE fma (sm_90 has no packed fp32 FMA)
+__device__ __forceinline__ float2 ffma2_rn(float2 a, float2 b, float2 c) {
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
 
 // slot s in 0..26 <-> offset d in {-1,0,1}^3 with s = (dx+1)*9 + (dy+1)*3 + (dz+1)

@@ -82,7 +82,7 @@ k_build_rows(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ xyz, co
 // ---- kernel rows, one warp per VOXEL (the default): all locations whose containing voxel on level l is u share u's
 // 27-stencil and its features, and they are contiguous (locations are Morton sorted).  The warp-per-location kernel
 // above re-gathers 27 feature rows per location and level -- 27 L1 wavefronts per channel load, the measured limit of
-// that kernel (r2b: ~110 cycles per (location, level) and SM); here the stencil and the features (C <= 16, as float4
+// that kernel; here the stencil and the features (C <= 16, as float4
 // registers) are fetched ONCE per voxel and the loop over the voxel's locations is ALU + shuffles + the row stores.
 // Same arithmetic, same order: bitwise the rows of k_build_rows.
 template <int MODE, int NC4>
@@ -233,8 +233,7 @@ k_evaluate(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ alpha, co
 // consecutive queries share their containing voxel on the coarse levels almost always and on the finest level about
 // half of the time.  One warp walks kEvalRun consecutive queries and keeps, per level, the containing voxel with its
 // 27 neighbours, their features (one float4) and coefficients in registers; a level is re-fetched only when the
-// query leaves the voxel.  k_evaluate re-gathers all of it per query and level (three 27-wavefront gathers each; r2e:
-// 114 ms for the two evaluations of one cfg4 extraction).  Same arithmetic in the same order: bitwise the values of
+// query leaves the voxel.  k_evaluate re-gathers all of it per query and level (three 27-wavefront gathers each).  Same arithmetic in the same order: bitwise the values of
 // k_evaluate<false>.
 constexpr int kEvalRun = 8;
 constexpr int kEvalMaxL = 4;

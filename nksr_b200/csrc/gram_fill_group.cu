@@ -36,7 +36,7 @@ __device__ __forceinline__ void accum_row(float (&R)[8][NLEV], const unsigned m8
       const float a = __shfl_sync(0xffffffffu, wl0, S + (c >> 2) * 9 + ((c >> 1) & 1) * 3 + (c & 1));
 #pragma unroll
       for (int k2 = 0; k2 + 1 < NLEV; k2 += 2) {
-        const float2 r = __ffma2_rn(make_float2(a, a), make_float2(ln[k2], ln[k2 + 1]),
+        const float2 r = ffma2_rn(make_float2(a, a), make_float2(ln[k2], ln[k2 + 1]),
                                     make_float2(R[c][k2], R[c][k2 + 1]));
         R[c][k2] = r.x;
         R[c][k2 + 1] = r.y;

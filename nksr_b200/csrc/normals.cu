@@ -173,7 +173,7 @@ k_knn_normals(const nksr_svh_t svh, const float* __restrict__ xyz, const float* 
     const float full = l + 1 < L ? hl * hl * 1.0000005f : 3.0e38f;
     // first try a tighter radius: for surface-like data the block's `total` points cover ~9 h^2, so ~1.7 k of them lie
     // within r^2 = 9 h^2 * 1.7 k / (pi * total); then the candidate buffer rarely overflows (one sort per point instead
-    // of two or three -- the bitonic network is this kernel's cost, r2f).  Too tight (fewer than k found): scan again.
+    // of two or three -- the bitonic network is this kernel's cost).  Too tight (fewer than k found): scan again.
     float first = 9.0f * hl * hl * (1.7f * (float)k) / (3.14159265f * (float)total);
     first = first < full ? first : full;
     float dk2 = 0.f;

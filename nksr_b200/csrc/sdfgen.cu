@@ -1,4 +1,4 @@
-// Ground-truth SDF from an oriented point cloud (SURVEY section 8(f) row 4): a from-scratch B200 replacement of the
+// Ground-truth SDF from an oriented point cloud (SURVEY section 8(f) row 4): a from-scratch sm_90a replacement of the
 // reference's only native code, ext/sdfgen/sdf_from_points.cu + the tinyflann kd-tree ext/common/kdtree_cuda.cu
 // (built by ext/__init__.py:18-23; call sites dataset/av_gt_geometry.py:63-78, models/loss.py:85).
 //

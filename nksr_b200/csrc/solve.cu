@@ -23,7 +23,7 @@ namespace {
 
 constexpr int kBlock = 256;
 constexpr int kWarpsPerBlock = kBlock / 32;
-constexpr int kGrid = 148 * 8;  // persistent-style grid: 8 blocks per SM (B200: 148 SMs)
+constexpr int kGrid = 132 * 8;  // persistent-style grid: 8 blocks per SM (H100 SXM: 132 SMs)
 
 // device-resident solver state (lives at the end of the caller's workspace)
 struct PcgCtrl {
@@ -52,8 +52,8 @@ k_spmv(const int64_t* __restrict__ rowptr, const int32_t* __restrict__ col, cons
   double local = 0.0;
   for (int64_t row = blockIdx.x * (int64_t)kWarpsPerBlock + wid; row < n; row += nwarps) {
     const int64_t b = __ldg(rowptr + row), e = __ldg(rowptr + row + 1);
-    // (prefetching the next row's pointers was tried: 10.4 ms instead of 7.45 ms, r2h -- the two loop-carried 64-bit
-    // values push the kernel past the 32 registers that keep the persistent 148 x 8 grid resident)
+    // (prefetching the next row's pointers was tried and measured slower -- the two loop-carried 64-bit
+    // values push the kernel past the 32 registers that keep the persistent 8-blocks-per-SM grid resident)
     // matrix stream: evict-first loads (read once per SpMV); x: read-only path, stays in L1/L2.
     // Four independent 128 B column + value requests per lane keep ~1 KB per warp in flight.
     float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
@@ -436,8 +436,8 @@ int nksr_spmv_stream(const int64_t* rowptr, const int32_t* col, const float* val
 namespace {
 
 // w = A u on the OWNED rows (others: w = 0); partials of (r,u), (w,u), (r,r) over the owned rows
-// (8 resident blocks per SM = 32 registers: the persistent 148 x 8 grid must fit in one wave -- at 40 registers it ran
-// in two, 12.1 ms per launch instead of 7.5, r2o)
+// (8 resident blocks per SM = 32 registers: the persistent 8-blocks-per-SM grid must fit in one wave -- at 40 registers it ran
+// in two and took half as long again)
 __global__ void __launch_bounds__(kBlock, 8)
 k_dcg_spmv(const int64_t* __restrict__ rowptr, const int32_t* __restrict__ col, const float* __restrict__ val,
            const uint8_t* __restrict__ owned, const float* __restrict__ r, const float* __restrict__ u,

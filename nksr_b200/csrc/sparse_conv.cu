@@ -15,8 +15,8 @@
 //   k_gather_gemm_tf32: mma.sync.m16n8k8 TF32 (fp32 accumulate), one 16 x TN strip per warp, operands staged by a
 //                       two-stage cp.async pipeline; inputs are rounded to TF32 (10-bit mantissa, cvt.rna), so results
 //                       differ from fp32 by ~1e-3 relative
-//   k_gather_gemm_tc  : tcgen05.mma kind::tf32, 128 x TN accumulator in TMEM (TN = 32 / 64 / 128), operands gathered by
-//                       cp.async into SWIZZLE_128B tiles, three-stage mbarrier ring -- the fast kernel (see below)
+//   k_gather_gemm_tc  : wgmma.mma_async tf32, two warpgroups x (64 x TN) register accumulators (TN = 32 / 64 / 128),
+//                       operands gathered by cp.async into 128-byte-swizzled tiles, four-stage ring -- see below
 #include "common.cuh"
 
 namespace {
@@ -264,99 +264,113 @@ int launch_tf32(dim3 grid, cudaStream_t s, const float* x, const int32_t* idx, i
 
 
 // ---------------------------------------------------------------------------------------------------------------------
-// k_gather_gemm_tc: the same gather-GEMM on the 5th-generation tensor cores (tcgen05.mma kind::tf32, accumulator in TMEM).
+// k_gather_gemm_tc: the same gather-GEMM on the Hopper tensor cores (wgmma.mma_async kind tf32, fp32 accumulator in
+// registers).
 //
 //   * A tile (128 gathered rows x 32 channels = 128 B per row) and B tile (TN output channels x 32 input channels; the
 //     caller passes W transposed to [K][c_out][c_in], "K-major" for the MMA) are written by cp.async straight into the
-//     canonical K-major SWIZZLE_128B shared-memory layout: row r at r * 128 B, its 16-byte chunk c at position
+//     canonical K-major 128-byte-swizzle shared-memory layout: row r at r * 128 B, its 16-byte chunk c at position
 //     c ^ (r & 7); 8-row groups 1024 B apart (the descriptor's stride byte offset).  Absent sources are zero-filled.
-//   * one thread issues 4 x tcgen05.mma (M = 128, N = TN, K = 8) per (offset, 32-channel chunk) step; the step's
-//     tcgen05.commit arrives on the stage's mbarrier, which is what lets the gather refill that stage: a three-stage
-//     ring, two steps of gathers in flight under the MMAs.
-//   * the accumulator (128 lanes x TN fp32 columns of TMEM) is read once, at the end: tcgen05.ld 32x32b (one row of 32
-//     columns per thread), bias / residual / ReLU in registers, 128-bit stores.
+//   * the two warpgroups of the CTA own rows 0-63 and 64-127; per (offset, 32-channel chunk) step each issues
+//     4 x wgmma (M = 64, N = TN, K = 8) on its half of the A tile and the whole B tile.  A four-stage ring keeps two
+//     steps of gathers in flight while the MMAs of the previous step may still run (wgmma.wait_group 1).
+//   * the accumulator (TN / 2 fp32 registers per thread, the m16n8 fragment layout repeated per 8 columns) goes through
+//     bias / residual / ReLU in registers and is stored as float2.
 // The operands are fp32 in shared memory; the tensor core reads their upper 19 bits (TF32).  W is rounded by the caller.
-constexpr int kTcStages = 3;
+constexpr int kTcStages = 4;
 constexpr int kTcATile = kTM * kKC * 4;        // 16 KB
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// shared-memory matrix descriptor, K-major SWIZZLE_128B (PTX ISA "tcgen05 matrix descriptor"): start address >> 4 in
-// bits [0,14), leading byte offset (unused for swizzled K-major; 1) in [16,30), stride byte offset 1024 >> 4 in [32,46),
-// version 1 in [46,48), base offset 0 (tiles are 1024-byte aligned), layout type 2 = SWIZZLE_128B in [61,64)
-__device__ __forceinline__ uint64_t tc_smem_desc(const uint32_t saddr) {
+// wgmma shared-memory matrix descriptor, K-major 128-byte swizzle (PTX ISA "matrix descriptor format" of
+// wgmma.mma_async): start address >> 4 in bits [0,14), leading byte offset (unused for swizzled K-major; 1) in [16,30),
+// stride byte offset 1024 >> 4 in [32,46), base offset 0 (tiles are 1024-byte aligned), swizzle mode 1 = 128 B in [62,64)
+__device__ __forceinline__ uint64_t wg_smem_desc(const uint32_t saddr) {
   const uint32_t lo = ((saddr & 0x3FFFFu) >> 4) | (1u << 16);
-  const uint32_t hi = (1024u >> 4) | (1u << 14) | (2u << 29);
+  const uint32_t hi = (1024u >> 4) | (1u << 30);
   return ((uint64_t)hi << 32) | lo;
 }
 
-// instruction descriptor of kind::tf32: D fp32 (bits [4,6) = 1), A and B TF32 ([7,10) = [10,13) = 2), both K-major
-// (bits 15, 16 = 0), N >> 3 in [17,23), M >> 4 in [24,29)
-template <int TN>
-__device__ __forceinline__ constexpr uint32_t tc_instr_desc() {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(kTM >> 4) << 24);
-}
-
-__device__ __forceinline__ void tc_mma_tf32(const uint32_t tmem_d, const uint64_t adesc, const uint64_t bdesc,
-                                            const uint32_t idesc, const uint32_t accumulate) {
+// D (64 x N, fp32 registers) (+)= A (64 x 8, tf32, smem) * B (8 x N, tf32, smem), N = 32 / 64 / 128
+__device__ __forceinline__ void wgmma_tf32(float (&d)[16], const uint64_t adesc, const uint64_t bdesc,
+                                           const uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+      "}, %16, %17, p, 1, 1;\n\t}\n"
+      :
+        "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
       : "memory");
 }
 
-__device__ __forceinline__ void mbar_wait_or_trap(const uint32_t bar, const uint32_t parity) {
-  // bounded: a commit that never arrives must end as a launch failure, not as a hung GPU
-  for (int i = 0; i < (1 << 24); ++i) {
-    uint32_t ok;
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-                 : "=r"(ok)
-                 : "r"(bar), "r"(parity)
-                 : "memory");
-    if (ok) return;
-  }
-  __trap();
+__device__ __forceinline__ void wgmma_tf32(float (&d)[32], const uint64_t adesc, const uint64_t bdesc,
+                                           const uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+      "}, %32, %33, p, 1, 1;\n\t}\n"
+      :
+        "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
+      : "memory");
+}
+
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], const uint64_t adesc, const uint64_t bdesc,
+                                           const uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1;\n\t}\n"
+      :
+        "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
+      : "memory");
 }
 
 template <int TN>
-__global__ void __launch_bounds__(kThreads, 2)
+__global__ void __launch_bounds__(kThreads, 1)
 k_gather_gemm_tc(const float* __restrict__ x, const int32_t* __restrict__ idx, int64_t n_out, int K,
                  const float* __restrict__ Wt, const float* __restrict__ bias, const float* __restrict__ res,
                  float* __restrict__ y, int Cin, int Cout, int relu) {
   constexpr int NS = kTcStages;
   constexpr int kBTile = TN * kKC * 4;
+  constexpr int kAHalf = kTcATile / 2;                        // 64 rows of the A tile: one warpgroup's operand
   extern __shared__ unsigned char smem_dyn[];
-  // SWIZZLE_128B atoms repeat every 1024 bytes and the descriptors carry base offset 0: align the tiles by hand
+  // 128-byte swizzle atoms repeat every 1024 bytes and the descriptors carry base offset 0: align the tiles by hand
   const uint32_t base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
   unsigned char* sm = smem_dyn + (base - smem_u32(smem_dyn));
   const uint32_t a_s = base;                                  // [NS][128 rows][128 B]
   const uint32_t b_s = base + NS * kTcATile;                  // [NS][TN rows][128 B]
   int32_t* src_s = reinterpret_cast<int32_t*>(sm + NS * (kTcATile + kBTile));   // [128][K]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sm + NS * (kTcATile + kBTile) + ((kTM * K * 4 + 15) & ~15));
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + NS);
-  unsigned* kmask_s = reinterpret_cast<unsigned*>(tmem_slot + 1);
+  unsigned* kmask_s = reinterpret_cast<unsigned*>(sm + NS * (kTcATile + kBTile) + ((kTM * K * 4 + 15) & ~15));
 
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const int wg = wid >> 2;                                    // warpgroup: rows 64 wg .. 64 wg + 63
   const int64_t row0 = (int64_t)blockIdx.x * kTM;
   const int n0 = blockIdx.y * TN;
   const int rows_here = (int)min((int64_t)kTM, n_out - row0);
 
-  if (tid == 0) {
-    *kmask_s = 0u;
-    for (int i = 0; i < NS; ++i)
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(bars + i)) : "memory");
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (wid == 0) {                              // one warp allocates the accumulator's TMEM columns (and frees them)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TN)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+  if (tid == 0) *kmask_s = 0u;
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_d = *tmem_slot;
   {
     unsigned mine = 0u;
     const int32_t* ip = idx + row0 * K;
@@ -399,98 +413,61 @@ k_gather_gemm_tc(const float* __restrict__ x, const int32_t* __restrict__ idx, i
     }
   };
 
-  for (int p = 0; p < NS - 1; ++p) {
+  float acc[TN / 2];
+#pragma unroll
+  for (int i = 0; i < TN / 2; ++i) acc[i] = 0.f;
+
+  constexpr int PF = NS - 2;                   // gather distance: stage (s + PF) % NS was last read by step s - 2
+  for (int p = 0; p < PF; ++p) {
     if (p < nsteps) issue(p);
     cp_async_commit();
   }
-  constexpr uint32_t idesc = tc_instr_desc<TN>();
   for (int s = 0; s < nsteps; ++s) {
-    const int pf = s + NS - 1;                 // its stage was read by the MMAs of step s - 1
-    if (pf < nsteps) {
-      if (s >= 1) mbar_wait_or_trap(smem_u32(bars + (s - 1) % NS), ((s - 1) / NS) & 1);
-      issue(pf);
-    }
-    cp_async_commit();
-    cp_async_wait<NS - 1>();                   // this thread's copies of step s have landed ...
+    cp_async_wait<PF - 1>();                   // this thread's copies of step s have landed ...
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // ... and are visible to the tensor core's proxy
+    // every thread's copies of step s are in; both warpgroups have retired the MMAs of step s - 2
     __syncthreads();
-    if (tid == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int buf = s % NS;
-      const uint64_t ad = tc_smem_desc(a_s + buf * kTcATile), bd = tc_smem_desc(b_s + buf * kBTile);
+    if (s + PF < nsteps) issue(s + PF);
+    cp_async_commit();
+    const int buf = s % NS;
+    const uint64_t ad = wg_smem_desc(a_s + buf * kTcATile + wg * kAHalf), bd = wg_smem_desc(b_s + buf * kBTile);
+    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll
-      for (int kk = 0; kk < kKC / 8; ++kk)     // 8 TF32 = 32 bytes along K inside the 128-byte swizzle row
-        tc_mma_tf32(tmem_d, ad + (uint64_t)(kk * 2), bd + (uint64_t)(kk * 2), idesc, (s | kk) != 0);
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                       smem_u32(bars + buf))
-                   : "memory");
-    }
+    for (int kk = 0; kk < kKC / 8; ++kk)       // 8 TF32 = 32 bytes along K inside the 128-byte swizzle row
+      wgmma_tf32(acc, ad + (uint64_t)(kk * 2), bd + (uint64_t)(kk * 2), (s | kk) != 0);
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+    asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
   }
+  asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
   cp_async_wait<0>();
-  // epilogue: warp w reads TMEM lanes 32 (w % 4) .. + 31 (its sub-partition); warps 0-3 take the first half of the
-  // columns, warps 4-7 the second (TN = 32: warps 0-3 take all), 32 columns = one 128-byte row segment at a time
-  constexpr int kColsPerWarp = TN >= 64 ? TN / 2 : 32;
-  const int colw = (wid >> 2) * kColsPerWarp;
-  if (nsteps > 0) {
-    mbar_wait_or_trap(smem_u32(bars + (nsteps - 1) % NS), ((nsteps - 1) / NS) & 1);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  }
-  const int64_t r = row0 + (wid & 3) * 32 + lane;
-  if (colw < TN) {
-#pragma unroll 1
-    for (int cc = 0; cc < kColsPerWarp; cc += 32) {
-      const int col0 = colw + cc;
-      float v[32];
+  // epilogue: warp w of the warpgroup holds rows 16 w + g and 16 w + g + 8 (g = lane / 4) of its 64, columns
+  // 8 j + 2 t, 8 j + 2 t + 1 (t = lane % 4) in acc[4 j .. 4 j + 3]
+  const int g = lane >> 2, t = lane & 3;
 #pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] = 0.f;
-      if (nsteps > 0) {
-        uint32_t u[32];
-        const uint32_t taddr = tmem_d + ((uint32_t)((wid & 3) * 32) << 16) + (uint32_t)col0;
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(u[0]), "=r"(u[1]), "=r"(u[2]), "=r"(u[3]), "=r"(u[4]), "=r"(u[5]), "=r"(u[6]), "=r"(u[7]), "=r"(u[8]),
-              "=r"(u[9]), "=r"(u[10]), "=r"(u[11]), "=r"(u[12]), "=r"(u[13]), "=r"(u[14]), "=r"(u[15]), "=r"(u[16]),
-              "=r"(u[17]), "=r"(u[18]), "=r"(u[19]), "=r"(u[20]), "=r"(u[21]), "=r"(u[22]), "=r"(u[23]), "=r"(u[24]),
-              "=r"(u[25]), "=r"(u[26]), "=r"(u[27]), "=r"(u[28]), "=r"(u[29]), "=r"(u[30]), "=r"(u[31])
-            : "r"(taddr)
-            : "memory");
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+  for (int h = 0; h < 2; ++h) {
+    const int64_t r = row0 + wg * 64 + (wid & 3) * 16 + g + 8 * h;
+    if (r >= n_out) continue;
 #pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(u[i]);
+    for (int j = 0; j < TN / 8; ++j) {
+      const int cidx = n0 + j * 8 + 2 * t;
+      float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+      if (bias) { v0 += __ldg(bias + cidx); v1 += __ldg(bias + cidx + 1); }
+      if (res) {
+        const float2 rv = __ldg(reinterpret_cast<const float2*>(res + r * Cout + cidx));
+        v0 += rv.x; v1 += rv.y;
       }
-      if (r < n_out) {
-        float* yp = y + r * Cout + n0 + col0;
-        const float* rp = res ? res + r * Cout + n0 + col0 : nullptr;
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          float4 o = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-          if (bias) {
-            const float4 bq = __ldg(reinterpret_cast<const float4*>(bias + n0 + col0) + q);
-            o.x += bq.x; o.y += bq.y; o.z += bq.z; o.w += bq.w;
-          }
-          if (rp) {
-            const float4 rq = __ldg(reinterpret_cast<const float4*>(rp) + q);
-            o.x += rq.x; o.y += rq.y; o.z += rq.z; o.w += rq.w;
-          }
-          if (relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); o.z = fmaxf(o.z, 0.f); o.w = fmaxf(o.w, 0.f); }
-          reinterpret_cast<float4*>(yp)[q] = o;
-        }
-      }
+      if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+      *reinterpret_cast<float2*>(y + r * Cout + cidx) = make_float2(v0, v1);
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (wid == 0)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "r"(TN) : "memory");
 }
 
 template <int TN>
 int launch_tc(dim3 grid, cudaStream_t s, const float* x, const int32_t* idx, int64_t n_out, int K, const float* Wt,
               const float* bias, const float* res, float* y, int c_in, int c_out, int relu) {
   const size_t smem = 1024 + (size_t)kTcStages * (kTcATile + TN * kKC * 4) + (((size_t)kTM * K * 4 + 15) & ~(size_t)15) +
-                      kTcStages * 8 + 16;
-  if (smem > 113 * 1024) return NKSR_E_INVALID;     // two CTAs per SM
+                      16;
+  if (smem > 227 * 1024) return NKSR_E_INVALID;     // the sm_90 limit per block
   if (cudaFuncSetAttribute(k_gather_gemm_tc<TN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
     return NKSR_E_CUDA;
   k_gather_gemm_tc<TN><<<grid, kThreads, smem, s>>>(x, idx, n_out, K, Wt, bias, res, y, c_in, c_out, relu);
@@ -511,9 +488,8 @@ int nksr_gather_gemm(const float* x, const int32_t* idx, int64_t n_out, int K, c
   const int tn = c_out % 64 == 0 ? 64 : 32;
   const dim3 grid((unsigned)((n_out + kTM - 1) / kTM), (unsigned)(c_out / tn));
   if (K > 32 && tf32) return NKSR_E_INVALID;           // the tile's offset mask is one 32-bit word
-  if (tf32 == 3) {                                     // tcgen05: W is [K][c_out][c_in], rounded to TF32
+  if (tf32 == 3) {                                     // wgmma: W is [K][c_out][c_in], rounded to TF32
     // 128 output channels per CTA where the layer is that wide: the gathered rows are fetched once per 128 columns
-    // (r2y: 100 K rows, 128 -> 128 channels: 0.36 ms against 0.60 ms with 64-column tiles, 0.89 ms for mma.sync)
     int rc;
     if (c_out % 128 == 0) {
       const dim3 g128(grid.x, (unsigned)(c_out / 128));

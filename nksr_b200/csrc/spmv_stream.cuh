@@ -1,4 +1,4 @@
-// Streaming CSR SpMV for sm_100a: the matrix never goes through the L1 / register path.
+// Streaming CSR SpMV for sm_90a: the matrix never goes through the L1 / register path.
 // (SURVEY section 8 row a4; the CG SpMV is the kernel BASELINE.json names for the HBM roofline.)
 //
 // The (col, val) stream is cut into fixed tiles of kTile entries.  One elected producer thread per CTA moves whole
@@ -8,12 +8,12 @@
 //   phase 1  every thread turns its share of the tile into products  val * x[col]  in place (the x gathers are
 //            the only global loads of the kernel, perfectly balanced, 8 independent gathers per thread);
 //   phase 2  one warp per row sums the row's products from shared memory in a fixed order and writes y.
-// (A one-phase consumer -- warp per row straight from shared memory, no CTA barrier, 24 warps -- was measured slower:
-// 3.1 TB/s on the short rows against 4.5 TB/s, r2g.)
+// (A one-phase consumer -- warp per row straight from shared memory, no CTA barrier, 24 warps -- was measured slower
+// on the short rows.)
 // A row cut by a tile boundary is owned by the tile it starts in; the tiles it continues into leave their part in
 // head[tile] and k_spmv_heads adds the parts in tile order -- no atomics, bitwise reproducible.
 // The memory pipeline (kStages x 36 KB per CTA, 2 CTAs per SM) is independent of what the warps are waiting for,
-// which is what the warp-per-row kernel lacked (ncu r1b: 22.7 warps stalled on the scoreboard per issue, DRAM 60 %).
+// which is what the warp-per-row kernel lacked (profiled: most warps stalled on the scoreboard, DRAM well below its peak).
 #pragma once
 #include "common.cuh"
 
@@ -22,7 +22,7 @@ namespace {
 constexpr int kTile = 4096;             // entries per tile: 16 KB of columns + 16 KB of values
 constexpr int kTileRows = 512;          // row pointers staged per tile (int64): 4 KB
 constexpr int kStages = 3;
-constexpr int kStreamWarps = 16;        // consumer warps per CTA (r2e: 8 warps left the x gathers latency bound)
+constexpr int kStreamWarps = 16;        // consumer warps per CTA (8 warps left the x gathers latency bound)
 constexpr int kStreamThreads = (kStreamWarps + 1) * 32;   // + the producer warp
 constexpr int kStreamCtasPerSm = 2;
 
@@ -136,8 +136,7 @@ k_spmv_stream(const int64_t* __restrict__ rowptr, const int32_t* __restrict__ co
     const int64_t e0 = t * kTile;
     const int cnt = (int)((nnz - e0 < kTile) ? (nnz - e0) : kTile);
     // phase 1: products in place.  All 16 column indices of the thread first, then 16 independent x gathers in flight,
-    // then the multiplies (a loop of  val[e] *= x[col[e]]  serialises on the shared-memory store: measured 17.7 ms per
-    // SpMV, 8 stalled warps per issue, r2d)
+    // then the multiplies (a loop of  val[e] *= x[col[e]]  serialises on the shared-memory store)
     {
       constexpr int kPer = kTile / (kStreamWarps * 32);
       int c[kPer];
@@ -264,7 +263,7 @@ static int spmv_stream_sm_count() {
   if (sms == 0) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
   }
   return sms;
 }

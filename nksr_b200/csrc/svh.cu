@@ -194,7 +194,7 @@ __global__ void k_row_ranges(const int32_t* __restrict__ base, int64_t m, int32_
 
 extern "C" {
 
-const char* nksr_version(void) { return "nksr_b200 0.1 (sm_100a)"; }
+const char* nksr_version(void) { return "nksr_b200 0.1 (sm_90a)"; }
 
 const char* nksr_error_string(int code) {
   switch (code) {

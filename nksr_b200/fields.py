@@ -30,7 +30,7 @@ from .svh import SparseFeatureHierarchy
 # "structural" = straight to the final slot from prefix tables (SPEC S6b).  solver_config['placement'] or the
 # NKSR_PLACEMENT environment variable override it.
 DEFAULT_PLACEMENT = "structural"
-# measured A/B pending on the B200 (r2w): until then the layout every parity test of this round ran on
+# the layout every parity test runs on unless a test selects the other
 DEFAULT_ROW_LAYOUT = "levels"
 
 
@@ -191,7 +191,7 @@ class KernelField(BaseField):
         e = torch.empty((m, svh.depth, width), dtype=torch.float32, device=dev)      # location-major
         # 'location' (default): one warp per location (any channel count); 'voxel': one warp per voxel, stencil +
         # features fetched once for all the voxel's locations (bitwise the same rows)
-        # (r2d, cfg4: voxel 46.8 ms, location 43.4 ms -- the per-level launches and the zero pass eat the saved gathers)
+        # ('voxel' saves gathers, but its per-level launches and zero pass cost about as much)
         rows = self.solver_config.get("rows") or os.environ.get("NKSR_ROWS") or "location"
         if rows == "voxel" and self.z[0].shape[1] in (4, 8, 16):
             call("nksr_build_rows_voxel", svh.view(), self.feat_view(), xs, base, ranges, m, mode,
@@ -212,7 +212,6 @@ class KernelField(BaseField):
         profile = int(bool(self.solver_config.get("profile")))
         # 'rows' (default): one warp per row with register loads (csrc/solve.cu); 'stream': the CSR arrays reach the SMs
         # as tiles moved by bulk async copies (TMA engine) into a shared-memory ring (csrc/spmv_stream.cuh)
-        # measured on cfg4 (profiles/r2g_summary.md): rows 7.45 ms per SpMV (0.717 of the copy peak), stream 7.96 ms
         spmv = self.solver_config.get("spmv") or os.environ.get("NKSR_SPMV") or "rows"
         if spmv not in ("stream", "rows"):
             raise ValueError("solver_config['spmv'] must be 'stream' or 'rows'")
@@ -267,7 +266,7 @@ class KernelField(BaseField):
             # transposed entries go straight to their final slot (SPEC S6b): per (fine level, offset) pair
             # a rank table on the fine level and a 125-ancestor prefix table on the coarse level
             cnt_down = torch.zeros(n, dtype=torch.int32, device=dev)
-            # row lengths with one column table per sibling group (r2d: 16 ms against 29 ms for a walk per slot and row)
+            # row lengths with one column table per sibling group (fewer lookups than a walk per slot and row)
             count = self.solver_config.get("count") or os.environ.get("NKSR_COUNT") or "grouped"
             grouped = count == "grouped" and svh.depth <= 4 and svh.depth < _lib.MAX_DEPTH
             call("nksr_gram_count_grouped" if grouped else "nksr_gram_count_own", svh.view(), cnt, st)
@@ -338,8 +337,7 @@ class KernelField(BaseField):
             normal_value = normal_value.detach().to(dev, torch.float32).contiguous()
             # approx_kernel_grad: compact gradient rows (one 128 B line per location and level)
             # compact gradient rows (one line instead of three per location and level) save 2/3 of
-            # the row memory but cost ALU in the assembly; measured slower on B200 (profiles/r1c),
-            # so they are opt-in for clouds that would not fit otherwise
+            # the row memory but cost ALU in the assembly, so they are opt-in for clouds that would not fit otherwise
             nrm_mode = 2 if (self.approx_kernel_grad and compact) else 1
             _, t_nrm, _, range_nrm, e_nrm = self._sorted_rows(normal_xyz, nrm_mode, normal_value, interleaved=ilv)
             cs.nrm_compact = 2 if ilv else int(nrm_mode == 2)          # the C struct's row-layout code
@@ -396,9 +394,8 @@ class KernelField(BaseField):
         diag = torch.zeros(n, dtype=torch.float32, device=dev)
         # numeric phase.  'rows' (default): one warp per matrix row (csrc/assemble.cu); 'grouped': one warp per
         # sibling group -- eight rows share their constraint lines, column tables and flush indices
-        # (csrc/gram_fill_group.cu).  Measured on cfg4 (profiles/r2d_summary.md): grouped 247 ms against 186 ms -- the
-        # sharing halves the loads but the per-sibling tests and flushes cost as many instructions as they save, and
-        # 13.4 KB of shared memory + 128 registers per warp leave 11 resident warps per SM instead of 30
+        # (csrc/gram_fill_group.cu).  The sharing halves the loads but the per-sibling tests and flushes cost as many
+        # instructions as they save, and 13.4 KB of shared memory + 128 registers per warp cut the resident warps per SM
         fill = self.solver_config.get("fill") or os.environ.get("NKSR_FILL") or "rows"
         if fill not in ("grouped", "rows"):
             raise ValueError("solver_config['fill'] must be 'grouped' or 'rows'")

@@ -73,7 +73,7 @@ class NKSRNetwork(nn.Module):
         self.backbone = str(hp["backbone"])
         if self.backbone not in ("pool", "unet"):
             raise ValueError("backbone: 'pool' or 'unet'")
-        # precision: 'fp32' (FFMA kernel), 'tf32' (mma.sync), 'tc' (tcgen05 + TMEM) -- csrc/sparse_conv.cu
+        # precision: 'fp32' (FFMA kernel), 'tf32' (mma.sync), 'tc' (wgmma tensor cores) -- csrc/sparse_conv.cu
         self.tf32 = {"tf32": True, "tc": 3}.get(str(hp["precision"]), False)
         interp = hp["interpolator"]
         gen = torch.Generator().manual_seed(int(hp["seed"]))
@@ -171,5 +171,5 @@ def load_checkpoint_from_url(url: str):
     import os
     if os.path.exists(url):
         return torch.load(url, map_location="cpu")
-    raise RuntimeError(f"cannot fetch checkpoint '{url}': no network access; the B200 build uses the seeded "
+    raise RuntimeError(f"cannot fetch checkpoint '{url}': no network access; this build uses the seeded "
                        "stand-in network (nksr_b200/network.py)")

@@ -309,7 +309,7 @@ class Reconstructor:
                  kernel_dim: int = 4):
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise _lib.NksrError("nksr_b200.Reconstructor needs a CUDA device (B200-only build, no CPU path)")
+            raise _lib.NksrError("nksr_b200.Reconstructor needs a CUDA device (CUDA-only build, no CPU path)")
         _lib.load()
         self.chunk_tmp_device = self.device
         self.tree_depth, self.adaptive_depth = tree_depth, adaptive_depth

@@ -11,7 +11,7 @@ pretrained checkpoint is a network download (models/nksr_net.py:36-38).
 Where the time goes is the 3x3x3 sparse convolution, and that is a hand-written kernel (csrc/sparse_conv.cu,
 `nksr_gather_gemm`): a gather-GEMM over the index tables the hierarchy already holds (nbr27 for the 3^3 stencil,
 child8 for the stride-2 convolution, a parent-by-octant table for the up-projection), fp32 FFMA, TF32 mma.sync, or TF32
-tcgen05.mma with the accumulator in TMEM (`precision='tc'`).  The skip concatenation is never materialised (the decoder
+wgmma.mma_async on the Hopper tensor cores (`precision='tc'`).  The skip concatenation is never materialised (the decoder
 convolution runs over its two inputs in turn).  Point-wise MLPs and the heads are dense library GEMMs (torch), as
 BASELINE.json's north_star keeps the network on PyTorch.
 
@@ -38,7 +38,7 @@ def round_tf32(w: torch.Tensor) -> torch.Tensor:
 def gather_gemm(x, idx, weight, bias=None, res=None, relu=False, tf32=False, impl="cuda"):
     """y[i] = act(bias + res[i] + sum_k x[idx[i, k]] @ weight[k]) over the valid (>= 0) entries of idx (n_out, K).
     tf32: False / 0 = fp32 FFMA kernel; True / 1 = TF32 mma.sync kernel; 2 = the same, `weight` already TF32-rounded;
-    3 = the tcgen05 kernel (TMEM accumulator), `weight` already TF32-rounded and transposed to (K, c_out, c_in)."""
+    3 = the wgmma kernel (register accumulator), `weight` already TF32-rounded and transposed to (K, c_out, c_in)."""
     n_out, K = idx.shape
     if int(tf32) == 3 and impl == "cuda":
         c_out, c_in = weight.shape[1], weight.shape[2]

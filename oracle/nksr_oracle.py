@@ -1,7 +1,7 @@
 """CPU oracle for the NKSR reconstruction hot path -- TEST INFRASTRUCTURE ONLY.
 
 PARITY UNPINNED: the reference ships this path as a closed wheel (SURVEY.md section 0 /
-section 8c); /root/reference holds no source, golden vector or known-answer test for it.
+section 8c); the reference tree holds no source, golden vector or known-answer test for it.
 This file is therefore a first-principles restatement of the algorithm fixed in
 DESIGN.md ("SPEC"), anchored on the reference's *call sites*:
 

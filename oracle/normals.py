@@ -8,7 +8,7 @@ Follows the reference's open CPU twin line by line (examples/recons_waymo_cpu.py
     :34-36 flip normals with  <view_dir, normal> < 0
     :38-39 keep |cos| > cos(85 deg)
 
-`point_cloud_utils` is a third-party dependency absent from /root/reference (environment.yml pins no
+`point_cloud_utils` is a third-party dependency absent from the reference tree (environment.yml pins no
 version); its published algorithm is restated here: the k nearest neighbours of a point INCLUDING the point
 itself, the 3x3 covariance of those neighbours about their mean, the unit eigenvector of the smallest
 eigenvalue.  Parity unpinned (no golden vectors in the reference).  scipy's cKDTree does the search.

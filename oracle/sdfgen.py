@@ -1,6 +1,6 @@
 """CPU restatement of the reference's GT-SDF generator -- TEST INFRASTRUCTURE ONLY (never imported by the product).
 
-Follows /root/reference/ext/sdfgen/sdf_from_points.cu line by line (the only native code of the reference tree,
+Follows the reference's ext/sdfgen/sdf_from_points.cu line by line (the only native code of the reference tree,
 built by ext/__init__.py:18-23; call sites dataset/av_gt_geometry.py:63-78 and models/loss.py:85):
 
   :150-166  kd-tree over ref_xyz; adaptive_knn > 0: ref_std[i] = mean over the adaptive_knn nearest reference points
@@ -13,8 +13,8 @@ built by ext/__init__.py:18-23; call sites dataset/av_gt_geometry.py:63-78 and m
             grad = sum n_k w_k / sum w_k
 
 Unlike the rest of oracle/, this restatement is PINNED: oracle/Makefile.ref compiles the unmodified reference sources
-into oracle/_ref/nksr_sdfgen_ref.so and tests/test_gpu_sdfgen.py checks both this file and the CUDA kernel against that
-binary on the GPU.  The k-NN search is exact (tinyflann eps = 0, ext/common/kdtree_cuda.cuh:34); scipy's cKDTree stands in.
+into oracle/_ref/nksr_sdfgen_ref.so, whose outputs on the test inputs are stored in tests/golden/sdfgen/, and
+tests/test_gpu_sdfgen.py checks both this file and the CUDA kernel against them on the GPU.  The k-NN search is exact (tinyflann eps = 0, ext/common/kdtree_cuda.cuh:34); scipy's cKDTree stands in.
 """
 from __future__ import annotations
 

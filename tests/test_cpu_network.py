@@ -80,7 +80,7 @@ def _toy_hierarchy(depth=3, seed=0):
 def test_fused_unet_glue_is_the_plain_unet(monkeypatch):
     """The GPU path of SparseUNet.forward never concatenates the skip connection (the decoder convolution runs over its
     two inputs in turn) and runs the up-projection as an 8-tap gather-GEMM over `up_table`; with the kernel call replaced
-    by the torch definition of the same arguments (weights un-transposed for the tcgen05 layout) it must give the plain
+    by the torch definition of the same arguments (weights un-transposed for the wgmma layout) it must give the plain
     formulation (torch.cat + per-octant loop), for every kernel flag's weight layout."""
     import nksr_b200.unet as U
     svh = _toy_hierarchy()

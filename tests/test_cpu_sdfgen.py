@@ -1,5 +1,5 @@
 """oracle/sdfgen.py (restatement of ext/sdfgen/sdf_from_points.cu) on the CPU: analytic checks of the rule itself.
-The comparison with the reference BINARY (oracle/_ref) needs a GPU: tests/test_gpu_sdfgen.py."""
+The comparison with the reference BINARY's stored outputs needs a GPU: tests/test_gpu_sdfgen.py."""
 import os
 
 import numpy as np
@@ -28,7 +28,8 @@ def test_sdf_of_a_sphere():
 def test_reference_build_recipe_exists_and_copies_nothing():
     """oracle/Makefile.ref compiles the reference sources WHERE THEY LIE (no copy in the repo) into oracle/_ref/"""
     mk = open(os.path.join(ROOT, "oracle", "Makefile.ref")).read()
-    assert "/root/reference/ext" in mk and "_ref/nksr_sdfgen_ref.so" in mk
+    assert "REF ?= $(NKSR_REFERENCE)/ext" in mk and "$(REF)/sdfgen/sdf_from_points.cu" in mk
+    assert "_ref/nksr_sdfgen_ref.so" in mk
     for dirpath, _, files in os.walk(ROOT):
         if "/.git" in dirpath or "/oracle/_ref" in dirpath or "gpurun_out" in dirpath:
             continue

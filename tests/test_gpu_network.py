@@ -79,7 +79,8 @@ def test_gather_gemm_edge_cases(cuda, tf32):
 @pytest.mark.parametrize("taps,c_in,c_out", [(27, 32, 32), (27, 64, 32), (27, 32, 64), (27, 128, 64), (8, 32, 64),
                                              (27, 32, 96), (27, 256, 256)])
 def test_gather_gemm_tcgen05_matches_torch(cuda, taps, c_in, c_out):
-    """the tcgen05 / TMEM kernel (tf32 = 3: operands read as TF32 by the tensor core, fp32 accumulation in TMEM) against
+    """the tensor-core kernel (tf32 = 3, written with wgmma on sm_90a; the name is from its first, tcgen05, version:
+    operands read as TF32 by the tensor core, fp32 accumulation in registers) against
     dense torch fp32, the same bound as the mma.sync TF32 kernel; also bitwise repeatable (one accumulation order)"""
     from nksr_b200.unet import gather_gemm, round_tf32
     svh, _ = _svh(cuda)
@@ -132,7 +133,8 @@ def test_unet_forward_matches_torch_reference(cuda):
 
 
 def test_unet_forward_tcgen05_matches_torch_reference(cuda):
-    """the whole backbone with every convolution on the tcgen05 kernel (precision='tc') against the torch fp32 modules"""
+    """the whole backbone with every convolution on the tensor-core kernel (precision='tc', wgmma on sm_90a; the name is
+    from its first, tcgen05, version) against the torch fp32 modules"""
     from nksr_b200.network import NKSRNetwork
     svh, xyz = _svh(cuda, n=20_000, depth=3)
     net = NKSRNetwork(dict(backbone="unet", tree_depth=3, kernel_dim=4, precision="tc")).to(cuda)

@@ -201,7 +201,7 @@ def test_chunked_reconstruction_blends_and_welds(cuda):
         bound = torch.maximum(bound, torch.where(wk > 0, jk, torch.zeros_like(jk)))
         n_blend += (wk > 0).float()
     assert float(n_blend.min()) >= 2                                           # every query sits in a cross-fade band
-    assert bool(((fa - fb).abs() <= bound + 0.01 * max(scale, 1e-6)).all())  # r2y: largest excess 3e-9, scale 0.073
+    assert bool(((fa - fb).abs() <= bound + 0.01 * max(scale, 1e-6)).all())
     # (the blend is NOT the un-chunked function value for value: a chunk's weights are normalised by ITS point counts,
     # models/nksr_net.py:103-111, so the data-to-regulariser balance differs; the zero level sets agree -- checked above)
     # chunk_tmp_device = cpu: the solved chunks wait in host memory, visit the GPU per evaluation, return to the host
@@ -210,5 +210,5 @@ def test_chunked_reconstruction_blends_and_welds(cuda):
     assert all(f_.svh.device.type == "cpu" and f_.alpha.device.type == "cpu" for f_ in parked.fields)
     mp = parked.extract_dual_mesh(mise_iter=1)
     assert all(f_.svh.device.type == "cpu" for f_ in parked.fields)
-    # same faces; the vertices move by the run-to-run difference of two solves to tol = 1e-5 (r2y: 4e-5 = 4e-4 voxels)
+    # same faces; the vertices move by the run-to-run difference of two solves to tol = 1e-5
     assert torch.equal(mp.f, mesh.f) and torch.allclose(mp.v, mesh.v, atol=1e-3)

@@ -1,12 +1,12 @@
-"""One reconstruct_global() of a bench workload on ONE GPU (world size 1: same step kernels, no collectives), for ncu
-launch lists of the distributed-CG kernels.  usage: python tools/profile_global.py [workload]"""
+"""One reconstruct_global() of a bench workload on ONE GPU (world size 1: same step kernels, no collectives), for
+profiler launch lists of the distributed-CG kernels.  usage: python tools/profile_global.py [workload]"""
 import os, sys, json
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import torch
 import bench, nksr_b200
 from nksr_b200 import dist_solve
-wl = sys.argv[1] if len(sys.argv) > 1 else "cfg4_outdoor_10M"
+wl = sys.argv[1] if len(sys.argv) > 1 else "cfg4_outdoor_5M"
 dev = torch.device("cuda:0")
 xyz, sensor = bench.make_cloud(wl, 4, 0)
 rec = nksr_b200.Reconstructor(dev)

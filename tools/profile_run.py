@@ -1,4 +1,4 @@
-"""One reconstruct() (+ optional mesh) of a bench workload, for ncu captures.
+"""One reconstruct() (+ optional mesh) of a bench workload, for profiler captures.
 usage: python tools/profile_run.py [workload] [points] [mesh]"""
 import os, sys, json
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
