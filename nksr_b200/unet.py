@@ -67,20 +67,16 @@ def gather_gemm(x, idx, weight, bias=None, res=None, relu=False, tf32=False, imp
     return y
 
 
-def kernel_weights(cache, name, weight, mode, splits=None):
+def kernel_weights(weight, mode, splits=None):
     """`weight` (K, c_in, c_out) in the form the kernel of `mode` takes, cut along c_in into `splits` parts (the inputs of
     a convolution over a channel concatenation): mode 0 as is; 1 / 2 rounded to TF32; 3 rounded and transposed to
-    (K, c_out, c_in).  Cached in `cache[name]` until the parameter is modified or moved."""
-    key = (int(mode), splits, weight._version, weight.data_ptr())
-    hit = cache.get(name)
-    if hit is None or hit[0] != key:
-        w = weight.detach()
-        if mode:
-            w = round_tf32(w)
-        parts = [w] if splits is None else list(torch.split(w, list(splits), dim=1))
-        parts = [(q.transpose(1, 2) if int(mode) == 3 else q).contiguous() for q in parts]
-        cache[name] = (key, parts)
-    return cache[name][1]
+    (K, c_out, c_in).  Rebuilt on every call: no key can tell that the parameter was written in place through `.data`
+    (EMA updates, weight surgery), which bumps no version counter, and the weights are at most a few MB."""
+    w = weight.detach()
+    if mode:
+        w = round_tf32(w)
+    parts = [w] if splits is None else list(torch.split(w, list(splits), dim=1))
+    return [(q.transpose(1, 2) if int(mode) == 3 else q).contiguous() for q in parts]
 
 
 _KERNEL_FLAG = {0: 0, 1: 2, 2: 2, 3: 3}          # the weights are always rounded on the host (flag 2), never per fragment
@@ -106,7 +102,6 @@ class SparseConv(nn.Module):
         self.bias = nn.Parameter(torch.zeros(c_out))
         bound = math.sqrt(6.0 / (taps * c_in))                       # He-uniform over the full stencil
         nn.init.uniform_(self.weight, -bound, bound)
-        self._wcache = {}
 
     def forward(self, x, idx, res=None, relu=True, tf32=False, impl="cuda"):
         parts = tuple(x) if isinstance(x, (tuple, list)) else (x,)
@@ -115,7 +110,7 @@ class SparseConv(nn.Module):
             return gather_gemm(xc, idx, self.weight, self.bias, res, relu, False, impl)
         mode = int(tf32)
         splits = tuple(int(q.shape[1]) for q in parts) if len(parts) > 1 else None
-        ws = kernel_weights(self._wcache, "w", self.weight, mode, splits)
+        ws = kernel_weights(self.weight, mode, splits)
         return conv_parts(parts, idx, ws, self.bias, res, relu, mode)
 
 
@@ -200,14 +195,13 @@ class SparseUNet(nn.Module):
             nn.init.uniform_(p, -math.sqrt(6.0 / p.shape[1]), math.sqrt(6.0 / p.shape[1]))
         self.dec = nn.ModuleList([SparseConv(27, 2 * ch[l], ch[l]) for l in range(depth - 1)])
         self.heads = nn.ModuleList([nn.Linear(ch[l], 6 + 2 * kernel_dim) for l in range(depth)])
-        self._wcache = {}
 
     def up_project(self, y_coarse, svh, l, tf32=False, impl="cuda"):
         """level l+1 -> level l: every child takes its parent's features through the weight of its octant.  On the GPU
         this is the gather-GEMM kernel again, 8 taps with one valid source per row (`up_table`); impl='torch' is the
         plain per-octant loop the tests compare it with."""
         if impl == "cuda":
-            ws = kernel_weights(self._wcache, f"up{l}", self.up[l], int(tf32))
+            ws = kernel_weights(self.up[l], int(tf32))
             return conv_parts((y_coarse,), up_table(svh, l), ws, None, None, False, int(tf32))
         n_l = svh.num_voxels(l)
         out = torch.zeros((n_l, self.channels[l]), device=y_coarse.device)

@@ -180,29 +180,80 @@ def _tent(tau):
     return w, dw
 
 
+def _bspline_abs(tau):
+    """_bspline with every signed sum replaced by the sum of the absolute values of its terms: the magnitude scale of
+    the weights (running-error analysis; it also covers a rounding of tau, e.g. 0.5 - tau near the support edge)"""
+    a = np.abs(tau)
+    w = np.stack([0.5 * (0.5 + a) ** 2, 0.75 + tau ** 2, 0.5 * (0.5 + a) ** 2], axis=-1)
+    dw = np.stack([0.5 + a, 2.0 * a, 0.5 + a], axis=-1)
+    return w, dw
+
+
+def _tent_abs(tau):
+    """_tent as sums of absolute values (see _bspline_abs)"""
+    pos = tau >= 0
+    a = np.abs(tau)
+    w = np.stack([np.where(pos, 0.0, a), 1.0 + a, np.where(pos, a, 0.0)], axis=-1)
+    return w, np.abs(_tent(tau)[1])
+
+
 def _prod3(wx, wy, wz):
     return (wx[:, :, None, None] * wy[:, None, :, None] * wz[:, None, None, :]).reshape(wx.shape[0], 27)
 
 
-def level_rows(svh: OracleSVH, l: int, xyz: np.ndarray, base: np.ndarray, z: np.ndarray,
-               want_grad: bool, approx_kernel_grad: bool):
-    """Kernel row entries of level l for M locations.
-
-    returns cols (M,27) int (-1 = none), K (M,27), and dK (M,3,27) if want_grad.
-    K_l(x, i) = B3((x-c_i)/W_l) * <phi_l(x), z_i>, phi_l = trilinear interpolation of z (SPEC S4).
-    Rows whose containing voxel is inactive have no entries at this level (SPEC S3).
-    """
+def _level_tau(svh: OracleSVH, l: int, xyz: np.ndarray, base: np.ndarray):
+    """neighbour table rows (M,27) (-1 = none) and local coordinates tau (M,3) in the containing voxel of level l"""
     M = xyz.shape[0]
-    W = svh.level_w(l)
     ok = base >= 0
     b = np.where(ok, base, 0)
     ijk = svh.ijk(l).astype(np.int64)
     nbr = svh.nbr27(l)[b] if svh.n(l) else np.full((M, 27), -1)
     nbr = np.where(ok[:, None], nbr, -1)
     cb = ijk[b] if svh.n(l) else np.zeros((M, 3), np.int64)
-    tau = xyz.astype(np.float64) / W - (cb + 0.5)
-    Bw, dBw = zip(*[_bspline(tau[:, a]) for a in range(3)])
-    Tw, dTw = zip(*[_tent(tau[:, a]) for a in range(3)])
+    return nbr, xyz.astype(np.float64) / svh.level_w(l) - (cb + 0.5)
+
+
+def tent_branch_ambiguous(svh: OracleSVH, xyz: np.ndarray, ulps: int = 4) -> np.ndarray:
+    """(M,) bool: locations where an fp32 tau within `ulps` ulps of the fp64 one falls on the other side of the snap
+    zone |tau| < 2^-12 of the tent derivative on some level.  There an fp32 evaluation may take the other (one-sided vs
+    symmetric) derivative, which is a different formula, not a rounding error."""
+    base = svh.locate(xyz)
+    amb = np.zeros(xyz.shape[0], bool)
+    for l in range(svh.depth):
+        if svh.n(l) == 0:
+            continue
+        _, tau = _level_tau(svh, l, xyz, base[l])
+        mid = np.abs(tau) < TENT_SNAP
+        t32 = tau.astype(np.float32)
+        for k in range(-ulps, ulps + 1):
+            near = (t32 + np.float32(k) * np.spacing(t32)).astype(np.float64)
+            amb |= np.any((np.abs(near) < TENT_SNAP) != mid, axis=1) & (base[l] >= 0)
+    return amb
+
+
+def level_rows(svh: OracleSVH, l: int, xyz: np.ndarray, base: np.ndarray, z: np.ndarray,
+               want_grad: bool, approx_kernel_grad: bool, abs_terms: bool = False):
+    """Kernel row entries of level l for M locations.
+
+    returns cols (M,27) int (-1 = none), K (M,27), and dK (M,3,27) if want_grad.
+    K_l(x, i) = B3((x-c_i)/W_l) * <phi_l(x), z_i>, phi_l = trilinear interpolation of z (SPEC S4).
+    Rows whose containing voxel is inactive have no entries at this level (SPEC S3).
+    abs_terms: also return Kabs, dKabs -- the same expressions with the B-spline and tent weights, their derivatives
+    and z replaced by their sums of absolute values: the scale of the rounding error of any evaluation of K, dK.
+    """
+    nbr, K, dK = _level_rows(svh, l, xyz, base, z, want_grad, approx_kernel_grad, _bspline, _tent)
+    if not abs_terms:
+        return nbr, K, dK
+    _, Ka, dKa = _level_rows(svh, l, xyz, base, np.abs(z), want_grad, approx_kernel_grad, _bspline_abs, _tent_abs)
+    return nbr, K, dK, Ka, dKa
+
+
+def _level_rows(svh, l, xyz, base, z, want_grad, approx_kernel_grad, bspline, tent):
+    M = xyz.shape[0]
+    W = svh.level_w(l)
+    nbr, tau = _level_tau(svh, l, xyz, base)
+    Bw, dBw = zip(*[bspline(tau[:, a]) for a in range(3)])
+    Tw, dTw = zip(*[tent(tau[:, a]) for a in range(3)])
     B3 = _prod3(*Bw)
     T3 = _prod3(*Tw)
     zn = np.where((nbr >= 0)[:, :, None], z[np.maximum(nbr, 0)], 0.0).astype(np.float64)  # (M,27,C)
@@ -227,42 +278,54 @@ def level_rows(svh: OracleSVH, l: int, xyz: np.ndarray, base: np.ndarray, z: np.
 
 
 def build_system(svh: OracleSVH, feats, pos_xyz, normal_xyz, normal_value,
-                 pos_weight, normal_weight, reg_weight, approx_kernel_grad=False):
+                 pos_weight, normal_weight, reg_weight, approx_kernel_grad=False, abs_terms=False):
     """A = E^T diag(w) E + reg*R,  b = E^T diag(w) t   (SPEC S5).
 
     E rows: one per position constraint (target 0, weight pos_weight) and three per normal
     constraint (d/dx, d/dy, d/dz of f at normal_xyz; target normal_value; weight normal_weight).
     R is block-diagonal per level: R_ii' = K_l(c_i', i) for |i-i'|_inf <= 1.
     Call site: models/nksr_net.py:100-112.
+    abs_terms: also return Aabs = |E|^T diag(w) |E| + reg*|R| and babs = |E|^T diag(w) |t|, where |E| holds the
+    abs-term rows (level_rows(abs_terms=True)) and |R| the regulariser of |z|: the per-entry error scales.
     """
     offs = svh.offsets()
     n = int(offs[-1])
     N, Kn = pos_xyz.shape[0], normal_xyz.shape[0]
-    rows, cols, vals = [], [], []
+    rows, cols, vals, avals = [], [], [], []
     base_p = svh.locate(pos_xyz)
     base_n = svh.locate(normal_xyz) if Kn else np.zeros((svh.depth, 0), np.int64)
     for l in range(svh.depth):
         if svh.n(l) == 0:
             continue
-        nbr, K, _ = level_rows(svh, l, pos_xyz, base_p[l], feats[l], False, approx_kernel_grad)
+        nbr, K, _, *ab = level_rows(svh, l, pos_xyz, base_p[l], feats[l], False, approx_kernel_grad, abs_terms)
         r = np.repeat(np.arange(N), 27).reshape(N, 27)
         m = nbr >= 0
         rows.append(r[m]); cols.append(nbr[m] + offs[l]); vals.append(K[m])
+        if abs_terms:
+            avals.append(ab[0][m])
         if Kn:
-            nbr, _, dK = level_rows(svh, l, normal_xyz, base_n[l], feats[l], True, approx_kernel_grad)
+            nbr, _, dK, *ab = level_rows(svh, l, normal_xyz, base_n[l], feats[l], True, approx_kernel_grad, abs_terms)
             m = nbr >= 0
             for a in range(3):
                 r = np.repeat(N + 3 * np.arange(Kn) + a, 27).reshape(Kn, 27)
                 rows.append(r[m]); cols.append(nbr[m] + offs[l]); vals.append(dK[:, a][m])
+                if abs_terms:
+                    avals.append(ab[1][:, a][m])
     M = N + 3 * Kn
-    E = sp.csr_matrix((np.concatenate(vals), (np.concatenate(rows), np.concatenate(cols))), shape=(M, n))
+    rows, cols = np.concatenate(rows), np.concatenate(cols)
+    E = sp.csr_matrix((np.concatenate(vals), (rows, cols)), shape=(M, n))
     w = np.concatenate([np.full(N, pos_weight, np.float64), np.full(3 * Kn, normal_weight, np.float64)])
     t = np.concatenate([np.zeros(N), np.asarray(normal_value, np.float64).reshape(-1)])
     EW = E.T.multiply(w[None, :]).tocsr()
     A = (EW @ E).tocsr()
     b = EW @ t
     A = A + reg_weight * build_regulariser(svh, feats)
-    return A.tocsr(), b, E
+    if not abs_terms:
+        return A.tocsr(), b, E
+    Ea = sp.csr_matrix((np.concatenate(avals), (rows, cols)), shape=(M, n))
+    EaW = Ea.T.multiply(np.abs(w)[None, :]).tocsr()
+    Aabs = (EaW @ Ea).tocsr() + abs(reg_weight) * build_regulariser(svh, [np.abs(f) for f in feats])
+    return A.tocsr(), b, E, Aabs.tocsr(), EaW @ np.abs(t)
 
 
 def build_regulariser(svh: OracleSVH, feats):
@@ -354,21 +417,31 @@ def pcg(A, b, tol=1e-5, max_iter=2000, x0=None, dtype=np.float64):
 
 
 # --------------------------------------------------------------------------- field evaluation
-def evaluate_f(svh: OracleSVH, feats, alpha, xyz, grad=False, approx_kernel_grad=False):
+def evaluate_f(svh: OracleSVH, feats, alpha, xyz, grad=False, approx_kernel_grad=False, abs_terms=False):
     """f(x) = sum_l [b_l(x) active] sum_{i in N27(b_l(x))} alpha_i K_l(x,i)  (SPEC S3/S4).
-    Call site: models/loss.py:189-198,225."""
+    Call site: models/loss.py:189-198,225.
+    abs_terms: also return fabs = sum |alpha_i| Kabs_l(x,i) (and gabs from dKabs), the per-query error scales; the
+    result is then (f, fabs) or (f, g, fabs, gabs)."""
     offs = svh.offsets()
     base = svh.locate(xyz)
     f = np.zeros(xyz.shape[0])
     g = np.zeros((xyz.shape[0], 3)) if grad else None
+    fa = np.zeros(xyz.shape[0])
+    ga = np.zeros((xyz.shape[0], 3)) if grad else None
     for l in range(svh.depth):
         if svh.n(l) == 0:
             continue
-        nbr, K, dK = level_rows(svh, l, xyz, base[l], feats[l], grad, approx_kernel_grad)
+        nbr, K, dK, *ab = level_rows(svh, l, xyz, base[l], feats[l], grad, approx_kernel_grad, abs_terms)
         a = np.where(nbr >= 0, alpha[np.maximum(nbr, 0) + offs[l]], 0.0)
         f += np.sum(a * K, axis=1)
         if grad:
             g += np.einsum('ms,mas->ma', a, dK)
+        if abs_terms:
+            fa += np.sum(np.abs(a) * ab[0], axis=1)
+            if grad:
+                ga += np.einsum('ms,mas->ma', np.abs(a), ab[1])
+    if abs_terms:
+        return (f, g, fa, ga) if grad else (f, fa)
     return (f, g) if grad else f
 
 

@@ -110,10 +110,39 @@ def test_fused_unet_glue_is_the_plain_unet(monkeypatch):
                 for name in ("structure", "normal", "basis", "udf", "decoder"):
                     a, b = getattr(out, name)[l], getattr(ref, name)[l]
                     assert float((a - b).abs().max()) <= tol * float(b.abs().max()), (mode, name, l)
-    # the prepared weights are cached until the parameter changes
-    w1 = U.kernel_weights(net.dec[0]._wcache, "w", net.dec[0].weight, 3, (32, 32))
-    assert U.kernel_weights(net.dec[0]._wcache, "w", net.dec[0].weight, 3, (32, 32)) is w1
+
+
+def test_kernel_weights_follow_in_place_writes(monkeypatch):
+    """The weights in kernel form (TF32-rounded, transposed for wgmma, split along c_in for the decoder's two inputs)
+    follow the parameter, also after a write through `.data` (EMA updates, weight surgery), which bumps no version
+    counter: the next forward of every kernel flag uses the new weights."""
+    import nksr_b200.unet as U
+    svh = _toy_hierarchy()
+    net = SparseUNet(3, 32, 4)
+    g = torch.Generator().manual_seed(2)
+    x0 = torch.randn((svh.num_voxels(0), 32), generator=g)
+    w1 = U.kernel_weights(net.dec[0].weight, 3, (32, 32))
     assert tuple(w1[0].shape) == (27, 32, 32) and w1[0].is_contiguous()
-    with torch.no_grad():
-        net.dec[0].weight.add_(1.0)
-    assert U.kernel_weights(net.dec[0]._wcache, "w", net.dec[0].weight, 3, (32, 32)) is not w1
+    assert torch.equal(w1[1], U.round_tf32(net.dec[0].weight.detach()[:, 32:]).transpose(1, 2))
+
+    def fake_kernel(x, idx, weight, bias=None, res=None, relu=False, tf32=False, impl="cuda"):
+        w = weight.transpose(1, 2) if int(tf32) == 3 else weight
+        return gather_gemm(x, idx, w, bias, res, relu, impl="torch")
+    monkeypatch.setattr(U, "gather_gemm", fake_kernel)
+    for mode, tol in ((False, 1e-5), (True, 2e-2), (3, 2e-2)):
+        with torch.no_grad():
+            net(x0, svh, tf32=mode)                                      # a forward with the old weights first
+            for q in net.parameters():
+                q.data.copy_(torch.randn(q.shape, generator=g) * 0.2)
+            out = net(x0, svh, tf32=mode)
+            ref = net(x0, svh, impl="torch")
+        for l in range(3):
+            a, b = out.decoder[l], ref.decoder[l]
+            assert float((a - b).abs().max()) <= tol * float(b.abs().max()), (mode, l)
+    new = torch.randn_like(net.dec[0].weight)
+    net.dec[0].weight.data.copy_(new)
+    for mode in (0, 1, 2, 3):
+        ws = U.kernel_weights(net.dec[0].weight, mode, (32, 32))
+        for w, part in zip(ws, (new[:, :32], new[:, 32:])):
+            part = U.round_tf32(part) if mode else part
+            assert torch.equal(w, part.transpose(1, 2) if mode == 3 else part)

@@ -8,6 +8,7 @@ import torch
 
 from oracle import nksr_oracle as O
 from tests import clouds
+from tests.bounds import KAPPA_FIELD, KAPPA_GRAM, KAPPA_RHS, assert_within, level_pair_label
 
 pytestmark = pytest.mark.gpu
 
@@ -37,18 +38,22 @@ def test_assembly_solve_mesh_at_depth(cuda, L, W, approx):
     field.solve(t(xyz), t(nxyz), t(nval), pw, nw, 1.0)
     s = field.system
     A = sp.csr_matrix((_np(s.val).astype(np.float64), _np(s.col), _np(s.rowptr)), shape=(s.n, s.n))
-    A_ref, b_ref, _ = O.build_system(osvh, feats, xyz, nxyz, nval, pw, nw, 1.0, approx)
+    # no constraint or query location within a few ulps of the tent derivative's snap-zone edge (none left out)
+    q = (xyz[:300] + 0.003).astype(np.float32)
+    assert int(O.tent_branch_ambiguous(osvh, nxyz).sum()) == 0 and int(O.tent_branch_ambiguous(osvh, q).sum()) == 0
+    A_ref, b_ref, _, A_abs, b_abs = O.build_system(osvh, feats, xyz, nxyz, nval, pw, nw, 1.0, approx, abs_terms=True)
     P = O.structural_pattern(osvh)
     assert A.nnz == P.nnz
-    assert abs(A - A_ref).max() <= 5e-4 * abs(A_ref).max()
-    assert np.abs(_np(s.rhs) - b_ref).max() <= 5e-4 * np.abs(b_ref).max()
+    what = f"L={L} approx={approx}"
+    assert_within(A, A_ref, A_abs, KAPPA_GRAM, f"Gram values ({what})", level_pair_label(osvh.offsets()))
+    assert_within(_np(s.rhs), b_ref, b_abs, KAPPA_RHS, f"rhs ({what})")
+    assert_within(_np(s.diag), A_ref.diagonal(), A_abs.diagonal(), KAPPA_GRAM, f"diagonal ({what})")
     alpha = _np(field.alpha).astype(np.float64)
     assert np.linalg.norm(A_ref @ alpha - b_ref) <= 2e-4 * np.linalg.norm(b_ref)
-    q = (xyz[:300] + 0.003).astype(np.float32)
-    fo, go = O.evaluate_f(osvh, feats, alpha, q, grad=True, approx_kernel_grad=approx)
+    fo, go, fa, ga = O.evaluate_f(osvh, feats, alpha, q, grad=True, approx_kernel_grad=approx, abs_terms=True)
     r = field.evaluate_f(t(q), grad=True)
-    assert np.abs(_np(r.value) - fo).max() <= 2e-3 * max(np.abs(fo).max(), 1e-6)
-    assert np.abs(_np(r.gradient) - go).max() <= 2e-3 * np.abs(go).max()
+    assert_within(_np(r.value), fo, fa, KAPPA_FIELD, f"f ({what})")
+    assert_within(_np(r.gradient), go, ga, KAPPA_FIELD, f"grad f ({what})")
     mesh = field.extract_dual_mesh(mise_iter=1)
     rad = np.linalg.norm(_np(mesh.v), axis=1)
     # (a single coarse level cannot place the surface accurately; parity with the oracle is asserted above)
@@ -75,14 +80,17 @@ def test_hierarchy_from_explicit_keys(cuda):
     field.solver_config.update(keep_system=True, max_iter=0)
     nxyz = osvh2.centers(0)
     nval = np.tile(np.array([[0.0, 0.0, 1.0]], np.float32), (nxyz.shape[0], 1))
+    assert int(O.tent_branch_ambiguous(osvh2, nxyz).sum()) == 0          # no location left out (test_gpu_parity)
     field.solve(t(xyz), t(nxyz), t(nval), 3.0, 0.02, 1.0)
     s = field.system
     A = sp.csr_matrix((_np(s.val).astype(np.float64), _np(s.col), _np(s.rowptr)), shape=(s.n, s.n))
-    A_ref, b_ref, _ = O.build_system(osvh2, feats, xyz, nxyz, nval, 3.0, 0.02, 1.0)
+    A_ref, b_ref, _, A_abs, b_abs = O.build_system(osvh2, feats, xyz, nxyz, nval, 3.0, 0.02, 1.0, abs_terms=True)
     assert A.nnz == O.structural_pattern(osvh2).nnz
-    assert abs(A - A_ref).max() <= 5e-4 * abs(A_ref).max()
+    assert_within(A, A_ref, A_abs, KAPPA_GRAM, "Gram values (explicit keys)", level_pair_label(osvh2.offsets()))
+    assert_within(_np(s.rhs), b_ref, b_abs, KAPPA_RHS, "rhs (explicit keys)")
+    assert_within(_np(s.diag), A_ref.diagonal(), A_abs.diagonal(), KAPPA_GRAM, "diagonal (explicit keys)")
     # points in the pruned half have no level-0 term (SPEC S3) on both sides
     q = xyz[xyz[:, 0] < -0.05][:200]
     field.alpha = t(rng.normal(size=s.n).astype(np.float32))
-    fo = O.evaluate_f(osvh2, feats, _np(field.alpha).astype(np.float64), q)
-    assert np.abs(_np(field.evaluate_f(t(q)).value) - fo).max() <= 2e-3 * max(np.abs(fo).max(), 1e-6)
+    fo, fa = O.evaluate_f(osvh2, feats, _np(field.alpha).astype(np.float64), q, abs_terms=True)
+    assert_within(_np(field.evaluate_f(t(q)).value), fo, fa, KAPPA_FIELD, "f (explicit keys)")

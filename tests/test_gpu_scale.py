@@ -6,7 +6,11 @@ level, the sort-free placement and the default graph-replayed PCG:
   * voxel keys of every level                                   bit-exact
   * CSR pattern: row lengths == SPEC S6 counts, no duplicates, sampled rows column-exact, oracle nonzeros
     all present                                                 exact
-  * CSR values, rhs, diagonal                                   <= 5e-4 of the largest entry
+  * CSR values, rhs, diagonal                                   <= RTOL_GRAM (4e-6) of the largest entry of the same
+                                                                level-pair block (rhs, diagonal: of the same level);
+                                                                the C++ restatement gives no per-entry magnitude
+                                                                scale, so the per-entry bounds of the smaller
+                                                                oracle tests (test_gpu_parity.py) are not used here
   * PCG solution (bench tolerance 1e-4) on the ORACLE's system  residual <= 2e-4 ||b||
   * f (and grad f) at 10 K queries                              evaluation <= 2e-3 of max |f| against the
                                                                 oracle evaluating the same coefficients
@@ -18,10 +22,12 @@ import torch
 
 from oracle import cpu_port as P
 from tests import scenes
+from tests.bounds import assert_blockwise
 
 pytestmark = pytest.mark.gpu
 
-RTOL_GRAM = 5e-4
+# max |diff| / max |ref| per level block; worst measured on an H100 (400 W): 9.9e-7 (rhs, cfg4_outdoor)
+RTOL_GRAM = 4e-6
 
 
 def _np(t):
@@ -72,12 +78,11 @@ def test_assembly_solve_evaluate_at_bench_scale(cuda, scene, approx):
     A.sum_duplicates()
     assert A.nnz == rowptr[-1], "duplicate column inside a row"
     # ---- values (entries absent from the oracle are structural zeros: the difference covers both sides)
-    scale = abs(A_ref).max()
-    D = (A - A_ref)
-    assert abs(D).max() <= RTOL_GRAM * scale
-    assert abs(A - A.T).max() <= 1e-6 * scale
-    assert np.abs(_np(s.rhs) - b_ref).max() <= RTOL_GRAM * np.abs(b_ref).max()
-    assert np.abs(_np(s.diag) - A_ref.diagonal()).max() <= RTOL_GRAM * scale
+    offs = osvh.offsets()
+    assert_blockwise(A, A_ref, offs, RTOL_GRAM, f"Gram values ({scene})")
+    assert abs(A - A.T).max() <= 1e-6 * abs(A_ref).max()
+    assert_blockwise(_np(s.rhs), b_ref, offs, RTOL_GRAM, f"rhs ({scene})")
+    assert_blockwise(_np(s.diag), A_ref.diagonal(), offs, RTOL_GRAM, f"diagonal ({scene})")
     # ---- the GPU solution solves the ORACLE's system to the requested tolerance
     alpha = _np(field.alpha)
     res = np.linalg.norm(A_ref @ alpha.astype(np.float64) - b_ref) / np.linalg.norm(b_ref)
