@@ -109,6 +109,21 @@ NKSR_API int nksr_pool_children(const int32_t* child8, const float* in, int64_t 
 NKSR_API int nksr_gather_gemm(const float* x, const int32_t* idx, int64_t n_out, int K, const float* W,
                      const float* bias, const float* res, float* y, int c_in, int c_out, int relu, int tf32,
                      void* stream);
+/* Backward of nksr_gather_gemm (csrc/sparse_conv_bwd.cu).  Weight gradient of the same convolution for the output
+ * gradient g (n_out x c_out, already multiplied by the activation's derivative):
+ *   dW[k] = sum_i [idx[i*K+k] >= 0] x[idx[i*K+k],:]^T g[i,:]   (K x c_in x c_out)    db = sum_i g[i,:] (db may be NULL)
+ * Deterministic (no atomics; rows cut into spans fixed by the shapes, fp32 over <= 256 rows, fp64 across them).
+ * tf32: 0 = fp32 FFMA; 1..3 = mma.sync TF32 with x and g rounded by cvt.rna.  Shape limits as nksr_gather_gemm;
+ * n_out = 0 gives zeros.  ws: nksr_gather_gemm_wgrad_workspace_bytes(...) bytes, else NKSR_E_WORKSPACE. */
+NKSR_API size_t nksr_gather_gemm_wgrad_workspace_bytes(int64_t n_out, int K, int c_in, int c_out, int tf32);
+NKSR_API int nksr_gather_gemm_wgrad(const float* x, const int32_t* idx, int64_t n_out, int K, const float* g,
+                           int c_in, int c_out, float* dW, float* db, void* ws, size_t ws_bytes, int tf32,
+                           void* stream);
+/* idx_t (n_src x K) = the transpose of a per-tap injective table idx (n_out x K): idx_t[j*K+k] = i iff idx[i*K+k] = j,
+ * -1 elsewhere.  The input gradient of the convolution over idx is nksr_gather_gemm over idx_t.  *status (device,
+ * zeroed by the caller) |= 1 when two rows share a (source, tap), |= 2 when a source is >= n_src. */
+NKSR_API int nksr_transpose_taps(const int32_t* idx, int64_t n_out, int K, int64_t n_src, int32_t* idx_t,
+                        int32_t* status, void* stream);
 /* first/last+1 sorted location of every level-l voxel: range[2*u], range[2*u+1] */
 NKSR_API int nksr_row_ranges(const int32_t* base_l, int64_t m, int32_t* range, int64_t n_l, void* stream);
 

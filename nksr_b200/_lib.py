@@ -66,6 +66,9 @@ _SIGNATURES = {
     "nksr_pool27": ("i", "ppqipp"),
     "nksr_pool_children": ("i", "ppqipp"),
     "nksr_gather_gemm": ("i", "ppqippppiiiip"),
+    "nksr_gather_gemm_wgrad_workspace_bytes": ("z", "qiiii"),
+    "nksr_gather_gemm_wgrad": ("i", "ppqipiipppzip"),
+    "nksr_transpose_taps": ("i", "pqiqppp"),
     "nksr_build_rows": ("i", "SFppqiipp"),
     "nksr_build_rows_voxel": ("i", "SFpppqiipp"),
     "nksr_gram_count": ("i", "Sppp"),

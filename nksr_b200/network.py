@@ -28,7 +28,7 @@ from .svh import SparseFeatureHierarchy
 
 _DEFAULTS = dict(kernel_dim=4, tree_depth=4, adaptive_depth=2, feature="normal",
                  interpolator=dict(n_hidden=2, hidden_dim=16), udf=dict(enabled=False), seed=0,
-                 unet=dict(f_maps=32), backbone="pool", precision="fp32")
+                 unet=dict(f_maps=32), backbone="pool", precision="fp32", trainable=False)
 
 
 def _get(hp, key, default):
@@ -75,6 +75,11 @@ class NKSRNetwork(nn.Module):
             raise ValueError("backbone: 'pool' or 'unet'")
         # precision: 'fp32' (FFMA kernel), 'tf32' (mma.sync), 'tc' (wgmma tensor cores) -- csrc/sparse_conv.cu
         self.tf32 = {"tf32": True, "tc": 3}.get(str(hp["precision"]), False)
+        # trainable: the U-Net backbone keeps requires_grad and encoder / unet follow the caller's grad mode (the sparse
+        # convolution's backward: csrc/sparse_conv_bwd.cu); by default every parameter is frozen and both run without grad
+        self.trainable = bool(hp["trainable"])
+        if self.trainable and self.backbone != "unet":
+            raise ValueError("trainable=True needs backbone='unet' (the 'pool' stand-in has nothing to train)")
         interp = hp["interpolator"]
         gen = torch.Generator().manual_seed(int(hp["seed"]))
         state = torch.random.get_rng_state()
@@ -98,12 +103,20 @@ class NKSRNetwork(nn.Module):
         finally:
             torch.random.set_rng_state(state)
         del gen
-        for p in self.parameters():
-            p.requires_grad_(False)
+        if not self.trainable:
+            for p in self.parameters():
+                p.requires_grad_(False)
+
+    def _grad_mode(self):
+        """the caller's grad mode for a trainable network, no grad otherwise"""
+        return torch.set_grad_enabled(self.trainable and torch.is_grad_enabled())
 
     # ---- encoder: pool point features into the voxels of every level ---------------------
-    @torch.no_grad()
     def encoder(self, xyz: torch.Tensor, feat, svh: SparseFeatureHierarchy, depth: int = 0):
+        with self._grad_mode():
+            return self._encoder(xyz, feat, svh, depth)
+
+    def _encoder(self, xyz, feat, svh, depth):
         from ._lib import call, stream_ptr
         if self.backbone == "unet":
             if feat is None and self.point_encoder.fc_in.in_features > 3:
@@ -130,8 +143,11 @@ class NKSRNetwork(nn.Module):
         return SimpleNamespace(svh=svh, pooled=pooled)
 
     # ---- "U-Net": heads on the pooled statistics; hierarchy passes through -----------------
-    @torch.no_grad()
     def unet(self, feat, svh: SparseFeatureHierarchy, adaptive_depth: int = None, gt_decoder_svh=None):
+        with self._grad_mode():
+            return self._unet(feat, svh, adaptive_depth, gt_decoder_svh)
+
+    def _unet(self, feat, svh, adaptive_depth, gt_decoder_svh):
         dec_svh = gt_decoder_svh if gt_decoder_svh is not None else svh
         C = self.kernel_dim
         if self.backbone == "unet":

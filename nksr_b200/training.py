@@ -1,0 +1,157 @@
+"""Training losses of the U-Net backbone that need only the network's backward (not a backward through the kernel
+solve): the structure loss and the UDF loss of the reference (models/loss.py:143-160 and :106-140), with the samplers
+and ground-truth transform of configs/default/train.yaml (supervision.structure_weight, supervision.udf,
+supervision.spatial.gt_band / gt_soft).
+
+    feat, dec_svh, _ = net.unet(net.encoder(xyz, normal, svh, 0), svh)
+    l_struct, per_level = structure_loss(feat.structure_features, dec_svh, gt_svh)
+    l_udf = udf_loss(net.udf_decoder, feat.udf_features, dec_svh, ref_xyz, ref_normal, voxel_size)
+
+Both are plain torch on top of the hierarchy's CUDA tables; the gradients flow into the network through the sparse
+convolution's backward kernels (nksr_b200/unet.py, csrc/sparse_conv_bwd.cu).
+"""
+from __future__ import annotations
+
+import torch
+import torch.nn.functional as F
+
+from .fields import NeuralField
+from .sdfgen import sdf_from_points
+from .svh import SparseFeatureHierarchy
+
+# configs/default/train.yaml: supervision.structure_weight, supervision.udf (weight, samplers), spatial.gt_band
+STRUCTURE_WEIGHT = 20.0
+UDF_WEIGHT = 150.0
+UDF_SAMPLERS = (dict(type="uniform", n_samples=80000, expand=1, expand_top=5),
+                dict(type="band", n_samples=20000, eps=0.5))
+GT_BAND = 1.0
+
+
+def structure_loss(structure_features, dec_svh: SparseFeatureHierarchy, gt_svh: SparseFeatureHierarchy):
+    """sum over the levels of the cross-entropy of the structure logits (n_l, 3) of the decoder hierarchy's voxels
+    against gt_svh.evaluate_voxel_status (0 absent, 1 leaf, 2 with children; models/loss.py:150-156).  Returns
+    (total, {level: loss}); levels without voxels are skipped."""
+    grids = dec_svh.grids
+    per_level = {}
+    for d, logits in structure_features.items():
+        if logits.shape[0] == 0:
+            continue
+        gt = gt_svh.evaluate_voxel_status(grids[d], d)
+        per_level[d] = F.cross_entropy(logits, gt)
+    total = sum(per_level.values()) if per_level else torch.zeros((), device=dec_svh.device)
+    return total, per_level
+
+
+def svh_samples(svh: SparseFeatureHierarchy, n: int, expand: int = 0, expand_top: int = 0, generator=None):
+    """n points uniform over the voxels of every level (models/loss.py:22-52): a voxel drawn uniformly from all levels'
+    voxels, then a point uniform inside it; a level's voxels are first dilated by `expand` (`expand_top` on the
+    coarsest level) when that is >= 3"""
+    dev = svh.device
+    coords, scales = [], []
+    grids = svh.grids
+    for d in range(svh.depth):
+        if grids[d] is None:
+            continue
+        ijk = grids[d].active_grid_coords().long()
+        e = expand if d != svh.depth - 1 else expand_top
+        if e >= 3:
+            o = torch.arange(-e // 2 + 1, e // 2 + 1, device=dev)
+            o = torch.stack(torch.meshgrid(o, o, o, indexing="ij"), dim=3).view(-1, 3)
+            ijk = torch.unique((ijk[:, None, :] + o[None]).view(-1, 3), dim=0)
+        coords.append(grids[d].grid_to_world(ijk))
+        scales.append(torch.full((ijk.shape[0],), grids[d].voxel_size, device=dev))
+    coords, scales = torch.cat(coords), torch.cat(scales)
+    pick = (torch.rand((n,), device=dev, generator=generator) * coords.shape[0]).long()
+    local = (torch.rand((n, 3), device=dev, generator=generator) - 0.5) * scales[pick, None]
+    return coords[pick] + local
+
+
+def band_samples(ref_xyz, ref_normal, n: int, eps: float, generator=None):
+    """n points displaced from random reference points along their normals by N(0, eps) (models/loss.py:60-66)"""
+    dev = ref_xyz.device
+    pick = (torch.rand((n,), device=dev, generator=generator) * ref_xyz.shape[0]).long()
+    return ref_xyz[pick] + ref_normal[pick] * torch.randn((n, 1), device=dev, generator=generator) * eps
+
+
+def transform_field(f, voxel_size, gt_band=GT_BAND):
+    """soft truncation tanh(f / T) T, T = gt_band * voxel_size (models/loss.py:68-80, gt_soft: true)"""
+    t = gt_band * voxel_size
+    return torch.tanh(f / t) * t
+
+
+def udf_samples(svh, ref_xyz, ref_normal, voxel_size, samplers=UDF_SAMPLERS, generator=None):
+    out = []
+    for s in samplers:
+        if s["type"] == "uniform":
+            out.append(svh_samples(svh, s["n_samples"], s["expand"], s["expand_top"], generator))
+        else:
+            out.append(band_samples(ref_xyz, ref_normal, s["n_samples"], s["eps"] * voxel_size, generator))
+    return torch.cat(out, 0)
+
+
+def udf_gt(q, ref_xyz, ref_normal, voxel_size, gt_band=GT_BAND):
+    """|transform(-sdf_from_points(q, ref, 8, 0.02))| (models/loss.py:84-86, 111-118)"""
+    sdf = -sdf_from_points(q, ref_xyz, ref_normal, 8, 0.02, False)[0]
+    return transform_field(sdf, voxel_size, gt_band).abs()
+
+
+def udf_loss(udf_decoder, udf_features, svh: SparseFeatureHierarchy, ref_xyz, ref_normal, voxel_size,
+             samplers=UDF_SAMPLERS, gt_band=GT_BAND, generator=None, q=None):
+    """mean |transform(pd) - gt| / voxel_size over the UDF samples (models/loss.py:120-140).  pd is the UDF NeuralField
+    evaluated differentiably as udf_decoder(NeuralField._interp(q)) on the finest level's UDF features (the decoder
+    takes kernel_dim inputs); `q` overrides the samplers."""
+    if q is None:
+        q = udf_samples(svh, ref_xyz, ref_normal, voxel_size, samplers, generator)
+    gt = udf_gt(q, ref_xyz, ref_normal, voxel_size, gt_band)
+    field = NeuralField(svh, udf_decoder, {0: udf_features[0]})
+    pd = udf_decoder(field._interp(q.to(torch.float32).contiguous())).reshape(-1)
+    return torch.mean((transform_field(pd, voxel_size, gt_band) - gt).abs()) / voxel_size
+
+
+class TrainingScene:
+    """one oriented cloud with its encoder hierarchy (point splatting) and ground-truth hierarchy (adaptive, from the
+    normals, models/nksr_net.py:175-179).  The decoder runs on the encoder hierarchy: the predicted-structure regime,
+    where all three structure classes occur."""
+
+    def __init__(self, xyz, normal, voxel_size, depth, adaptive_depth=2):
+        dev = xyz.device
+        self.xyz, self.normal, self.voxel_size = xyz.contiguous(), normal.contiguous(), float(voxel_size)
+        self.enc_svh = SparseFeatureHierarchy(voxel_size, depth, dev).build_point_splatting(self.xyz)
+        self.gt_svh = SparseFeatureHierarchy(voxel_size, depth, dev).build_adaptive_normal_variation(
+            self.xyz, self.normal, adaptive_depth=adaptive_depth)
+        self.adaptive_depth = adaptive_depth
+
+
+def losses(net, scene: TrainingScene, generator=None):
+    """forward of a trainable NKSRNetwork on the scene and its weighted losses: (total, structure, udf)"""
+    enc = net.encoder(scene.xyz, scene.normal, scene.enc_svh, 0)
+    feat, dec_svh, _ = net.unet(enc, scene.enc_svh, adaptive_depth=scene.adaptive_depth)
+    l_struct, _ = structure_loss(feat.structure_features, dec_svh, scene.gt_svh)
+    l_udf = udf_loss(net.udf_decoder, feat.udf_features, dec_svh, scene.xyz, scene.normal, scene.voxel_size,
+                     generator=generator)
+    return STRUCTURE_WEIGHT * l_struct + UDF_WEIGHT * l_udf, l_struct, l_udf
+
+
+GRAD_CLIP = 0.5         # configs/default/train.yaml: grad_clip
+LEARNING_RATE = 1e-4    # configs/default/train.yaml: learning_rate.init
+
+
+def make_optimizer(net):
+    return torch.optim.Adam([p for p in net.parameters() if p.requires_grad], lr=LEARNING_RATE)
+
+
+def train_step(net, opt, scene: TrainingScene, generator=None, marks=None):
+    """one Adam step (gradient norm clipped to GRAD_CLIP); returns the (structure, udf) losses as tensors.  `marks`,
+    if given, is called with 'forward' / 'backward' / 'step' after each phase has been enqueued."""
+    opt.zero_grad(set_to_none=True)
+    total, l_struct, l_udf = losses(net, scene, generator)
+    if marks:
+        marks("forward")
+    total.backward()
+    if marks:
+        marks("backward")
+    torch.nn.utils.clip_grad_norm_([p for p in net.parameters() if p.requires_grad], GRAD_CLIP)
+    opt.step()
+    if marks:
+        marks("step")
+    return l_struct.detach(), l_udf.detach()

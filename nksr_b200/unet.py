@@ -27,7 +27,7 @@ from types import SimpleNamespace
 import torch
 from torch import nn
 
-from ._lib import call, stream_ptr
+from ._lib import NksrError, _ws, call, stream_ptr
 
 
 def round_tf32(w: torch.Tensor) -> torch.Tensor:
@@ -46,7 +46,7 @@ def gather_gemm(x, idx, weight, bias=None, res=None, relu=False, tf32=False, imp
         c_in, c_out = weight.shape[1], weight.shape[2]
     assert weight.shape[0] == K and x.shape[1] == c_in
     if impl == "torch":
-        y = torch.zeros((n_out, c_out), dtype=torch.float32, device=x.device)
+        y = torch.zeros((n_out, c_out), dtype=x.dtype, device=x.device)
         if bias is not None:
             y += bias
         if res is not None:
@@ -67,16 +67,78 @@ def gather_gemm(x, idx, weight, bias=None, res=None, relu=False, tf32=False, imp
     return y
 
 
-def kernel_weights(weight, mode, splits=None):
+def kernel_weights(weight, mode, splits=None, transposed=False):
     """`weight` (K, c_in, c_out) in the form the kernel of `mode` takes, cut along c_in into `splits` parts (the inputs of
     a convolution over a channel concatenation): mode 0 as is; 1 / 2 rounded to TF32; 3 rounded and transposed to
-    (K, c_out, c_in).  Rebuilt on every call: no key can tell that the parameter was written in place through `.data`
-    (EMA updates, weight surgery), which bumps no version counter, and the weights are at most a few MB."""
+    (K, c_out, c_in).  transposed=True gives the per-tap transposes W_k^T the input gradient runs the same kernel with:
+    (K, c_out, c_in) for modes 0-2, rounded (K, c_in, c_out) for mode 3.  Rebuilt on every call: no key can tell that the
+    parameter was written in place through `.data` (EMA updates, weight surgery), which bumps no version counter, and
+    the weights are at most a few MB."""
     w = weight.detach()
     if mode:
         w = round_tf32(w)
     parts = [w] if splits is None else list(torch.split(w, list(splits), dim=1))
-    return [(q.transpose(1, 2) if int(mode) == 3 else q).contiguous() for q in parts]
+    flip = (int(mode) == 3) != bool(transposed)
+    return [(q.transpose(1, 2) if flip else q).contiguous() for q in parts]
+
+
+def gather_gemm_wgrad(x, idx, g, tf32=False, bias=True, impl="cuda"):
+    """weight and bias gradient of `gather_gemm` for the output gradient g (n_out, c_out) (already through the
+    activation's derivative): dW[k] = sum_i [idx[i, k] >= 0] x[idx[i, k]]^T g[i]  (K, c_in, c_out), db = sum_i g[i]
+    (None unless `bias`).  tf32: 0 = fp32 FFMA, 1..3 = TF32 mma.sync (x and g rounded); deterministic
+    (csrc/sparse_conv_bwd.cu).  impl='torch' is the definition."""
+    n_out, K = idx.shape
+    c_in, c_out = x.shape[1], g.shape[1]
+    if impl == "torch":
+        xp = torch.cat([x, x.new_zeros((1, c_in))])                 # row -1 -> zeros
+        dw = torch.stack([xp[idx[:, k].long()].transpose(0, 1) @ g for k in range(K)]) if n_out else \
+            x.new_zeros((K, c_in, c_out))
+        return dw, (g.sum(dim=0) if bias else None)
+    x, idx, g = x.contiguous(), idx.contiguous(), g.contiguous()
+    dw = torch.empty((K, c_in, c_out), dtype=torch.float32, device=x.device)
+    db = torch.empty(c_out, dtype=torch.float32, device=x.device) if bias else None
+    nb = call("nksr_gather_gemm_wgrad_workspace_bytes", n_out, K, c_in, c_out, int(tf32))
+    ws = _ws(nb, x.device)
+    call("nksr_gather_gemm_wgrad", x, idx, n_out, K, g, c_in, c_out, dw, db, ws, nb, int(tf32), stream_ptr(x.device))
+    return dw, db
+
+
+def transpose_taps(idx, n_src, impl="cuda"):
+    """(n_src, K) int32 transpose of a gather table that is injective per tap: idx_t[j, k] = i iff idx[i, k] = j, -1
+    elsewhere.  The input gradient of a convolution over idx is the convolution over idx_t with W_k^T.  A table with a
+    repeated (source, tap) or a source >= n_src raises NksrError."""
+    n_out, K = idx.shape
+    if impl == "torch":
+        ok = idx >= 0
+        rows = torch.arange(n_out, device=idx.device)[:, None].expand(n_out, K)[ok]
+        key = idx.long()[ok] * K + torch.arange(K, device=idx.device)[None, :].expand(n_out, K)[ok]
+        if key.numel() and (int(key.max()) >= n_src * K or key.unique().numel() != key.numel()):
+            raise NksrError("transpose_taps: the table is not injective per tap or a source is out of range")
+        idx_t = torch.full((n_src * K,), -1, dtype=torch.int32, device=idx.device)
+        idx_t[key] = rows.to(torch.int32)
+        return idx_t.view(n_src, K)
+    idx = idx.contiguous()
+    idx_t = torch.empty((n_src, K), dtype=torch.int32, device=idx.device)
+    status = torch.zeros(1, dtype=torch.int32, device=idx.device)
+    call("nksr_transpose_taps", idx, n_out, K, n_src, idx_t, status, stream_ptr(idx.device))
+    st = int(status.item())
+    if st:
+        raise NksrError(f"nksr_transpose_taps: " + ("a (source, tap) pair occurs twice; " if st & 1 else "") +
+                        ("a source index is >= n_src" if st & 2 else "").rstrip("; "))
+    return idx_t
+
+
+def transposed_table(svh, idx, n_src):
+    """`transpose_taps(idx, n_src)`, cached on the hierarchy object while `idx` is alive (the rule of `up_table`: a weak
+    reference to the very tensor it was derived from, so a rebuilt table or a recycled id cannot pass for the old one)"""
+    cache = svh.__dict__.setdefault("_unet_transposes", {})
+    key = (id(idx), int(n_src))
+    hit = cache.get(key)
+    if hit is None or hit[0]() is not idx:
+        for stale in [k for k, v in cache.items() if v[0]() is None]:
+            del cache[stale]
+        cache[key] = (weakref.ref(idx), transpose_taps(idx, n_src))
+    return cache[key][1]
 
 
 _KERNEL_FLAG = {0: 0, 1: 2, 2: 2, 3: 3}          # the weights are always rounded on the host (flag 2), never per fragment
@@ -92,9 +154,59 @@ def conv_parts(parts, idx, weights, bias, res, relu, mode):
     return y
 
 
+class GatherConv(torch.autograd.Function):
+    """Autograd of `conv_parts` with the weight in parameter layout (K, sum_p c_p, c_out).  The forward is `conv_parts`
+    itself (the same kernels and bits as without grad).  Backward, with g = dY * [y > 0] under ReLU (relu'(0) = 0):
+      d_res = g,  d_bias = sum_i g[i],  dW = the weight-gradient kernel per part, concatenated along c_in,
+      d_part_p = the forward kernel over the transposed table with part p's slice of W_k^T.
+    idx_t: the transposed table, a function returning it (called once, in backward), or None (computed in backward)."""
+
+    @staticmethod
+    def forward(ctx, idx, idx_t, mode, relu, weight, bias, res, *parts):
+        splits = tuple(int(q.shape[1]) for q in parts) if len(parts) > 1 else None
+        y = conv_parts(parts, idx, kernel_weights(weight, mode, splits), bias, res, relu, mode)
+        ctx.idx, ctx.idx_t, ctx.mode, ctx.relu, ctx.splits = idx, idx_t, int(mode), bool(relu), splits
+        ctx.save_for_backward(weight, y if relu else None, *parts)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        weight, y, *parts = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        g = dy.contiguous()
+        if ctx.relu:
+            g = g * (y > 0)
+        d_w = d_b = d_res = None
+        if need[6]:
+            d_res = g
+        if need[4] or need[5]:
+            dws = []
+            for p, x in enumerate(parts):
+                dw, db = gather_gemm_wgrad(x, ctx.idx, g, ctx.mode, bias=p == 0 and need[5])
+                dws.append(dw)
+                d_b = db if p == 0 else d_b
+            d_w = dws[0] if len(dws) == 1 else torch.cat(dws, dim=1)
+        d_parts = [None] * len(parts)
+        if any(need[7:]):
+            idx_t = ctx.idx_t() if callable(ctx.idx_t) else ctx.idx_t
+            if idx_t is None:
+                idx_t = transpose_taps(ctx.idx, parts[0].shape[0])
+            wts = kernel_weights(weight, ctx.mode, ctx.splits, transposed=True)
+            for p in range(len(parts)):
+                if need[7 + p]:
+                    d_parts[p] = gather_gemm(g, idx_t, wts[p], None, None, False, _KERNEL_FLAG[ctx.mode])
+        return (None, None, None, None, d_w, d_b, d_res, *d_parts)
+
+
+def _wants_grad(*tensors):
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors)
+
+
 class SparseConv(nn.Module):
     """K-tap sparse convolution: weight (K, c_in, c_out) + bias; the taps' sources come from an index table.  `x` may be
-    a tuple of tensors: the convolution then runs over their channel concatenation (the U-Net's skip connections)."""
+    a tuple of tensors: the convolution then runs over their channel concatenation (the U-Net's skip connections).
+    With grad enabled and an input or parameter that requires grad, the CUDA path runs through `GatherConv`; `idx_t`
+    (the transposed table or a function returning it) saves its computation in backward."""
 
     def __init__(self, taps, c_in, c_out):
         super().__init__()
@@ -103,12 +215,14 @@ class SparseConv(nn.Module):
         bound = math.sqrt(6.0 / (taps * c_in))                       # He-uniform over the full stencil
         nn.init.uniform_(self.weight, -bound, bound)
 
-    def forward(self, x, idx, res=None, relu=True, tf32=False, impl="cuda"):
+    def forward(self, x, idx, res=None, relu=True, tf32=False, impl="cuda", idx_t=None):
         parts = tuple(x) if isinstance(x, (tuple, list)) else (x,)
         if impl != "cuda":
             xc = parts[0] if len(parts) == 1 else torch.cat(parts, dim=1)
             return gather_gemm(xc, idx, self.weight, self.bias, res, relu, False, impl)
         mode = int(tf32)
+        if _wants_grad(self.weight, self.bias, res, *parts):
+            return GatherConv.apply(idx, idx_t, mode, relu, self.weight, self.bias, res, *parts)
         splits = tuple(int(q.shape[1]) for q in parts) if len(parts) > 1 else None
         ws = kernel_weights(self.weight, mode, splits)
         return conv_parts(parts, idx, ws, self.bias, res, relu, mode)
@@ -201,10 +315,15 @@ class SparseUNet(nn.Module):
         this is the gather-GEMM kernel again, 8 taps with one valid source per row (`up_table`); impl='torch' is the
         plain per-octant loop the tests compare it with."""
         if impl == "cuda":
+            idx = up_table(svh, l)
+            if _wants_grad(self.up[l], y_coarse):
+                n_src = svh.num_voxels(l + 1)
+                return GatherConv.apply(idx, lambda: transposed_table(svh, idx, n_src), int(tf32), False, self.up[l],
+                                        None, None, y_coarse)
             ws = kernel_weights(self.up[l], int(tf32))
-            return conv_parts((y_coarse,), up_table(svh, l), ws, None, None, False, int(tf32))
+            return conv_parts((y_coarse,), idx, ws, None, None, False, int(tf32))
         n_l = svh.num_voxels(l)
-        out = torch.zeros((n_l, self.channels[l]), device=y_coarse.device)
+        out = torch.zeros((n_l, self.channels[l]), dtype=y_coarse.dtype, device=y_coarse.device)
         octant = octant_of_children(svh.child8[l + 1], n_l)
         parent = svh.parent[l].long()
         for o in range(8):
@@ -217,19 +336,21 @@ class SparseUNet(nn.Module):
         D = min(self.depth, svh.depth)
         kw = dict(tf32=tf32, impl=impl)
         xs, x = [], x0
+        # transposed tables for the input gradients, built on first use in backward and cached on the hierarchy
+        tt = lambda idx, l: (lambda: transposed_table(svh, idx, svh.num_voxels(l))) if impl == "cuda" else None
         for l in range(D):
             nbr = svh.nbr27[l]
-            h = self.enc_a[l](x, nbr, relu=True, **kw)
-            x = self.enc_b[l](h, nbr, res=x, relu=True, **kw)
+            h = self.enc_a[l](x, nbr, relu=True, idx_t=tt(nbr, l), **kw)
+            x = self.enc_b[l](h, nbr, res=x, relu=True, idx_t=tt(nbr, l), **kw)
             xs.append(x)
             if l + 1 < D:
-                x = self.down[l](x, svh.child8[l + 1], relu=True, **kw)
+                x = self.down[l](x, svh.child8[l + 1], relu=True, idx_t=tt(svh.child8[l + 1], l), **kw)
         ys = [None] * D
         y = xs[D - 1]
         ys[D - 1] = y
         for l in range(D - 2, -1, -1):
             u = self.up_project(y, svh, l, **kw)
-            y = self.dec[l]((xs[l], u), svh.nbr27[l], relu=True, **kw)         # conv over [skip ; up], not concatenated
+            y = self.dec[l]((xs[l], u), svh.nbr27[l], relu=True, idx_t=tt(svh.nbr27[l], l), **kw)   # [skip ; up], not cat
             ys[l] = y
         C = self.kernel_dim
         out = SimpleNamespace(structure={}, normal={}, basis={}, udf={}, decoder={})

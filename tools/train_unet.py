@@ -1,0 +1,151 @@
+"""Train the sparse-conv U-Net backbone (NKSRNetwork(backbone='unet', trainable=True)) on a seeded synthetic scene with
+the structure and UDF losses (nksr_b200/training.py), Adam lr 1e-4, gradient norm clipped to 0.5 (train.yaml).
+
+    python tools/train_unet.py --scene sphere --points 200000 --steps 30 --precision fp32 --out ckpt.pt
+    python tools/train_unet.py --scene cfg4 --points 1000000 --depth 4 --precision tc --steps 10
+
+Scenes: 'sphere' (tests/clouds.py, exact normals) or 'cfg4' (a crop of bench.py's outdoor scene at its own density,
+normals from the kNN preprocess).  Every step prints one JSON line: the losses and the CUDA-event times of the forward,
+the backward (with the sparse convolution's input-gradient and weight-gradient kernels separately) and the optimizer
+step.  The last line is a summary over the steps after the first two: median times, the weight-gradient kernel's
+achieved TFLOP/s (2 nnz_taps c_in c_out per call) and GB/s per (c_in, c_out) shape, and the GPU's name and power limit.
+--out saves {'state_dict': ...}, which load_checkpoint_from_url(<path>) + load_state_dict take."""
+import argparse
+import json
+import os
+import statistics
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if ROOT not in sys.path:
+    sys.path.insert(0, ROOT)
+os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")
+
+
+def make_scene(kind, n, depth, device):
+    import numpy as np
+    import torch
+    from nksr_b200.training import TrainingScene
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(device)
+    if kind == "sphere":
+        from tests import clouds
+        xyz, nrm = clouds.sphere(n, noise=0.001)
+        return TrainingScene(t(xyz), t(nrm), 0.02 if n <= 300_000 else 0.01, depth)
+    import nksr_b200
+    from tests import scenes
+    xyz, sensor, W = scenes.crop("cfg4_outdoor", n, with_sensor=True)
+    px, pn, _ = nksr_b200.get_estimate_normal_preprocess_fn(64, 85.0)(t(xyz), None, t(sensor))
+    return TrainingScene(px, pn, W, depth)
+
+
+class KernelTimer:
+    """CUDA events around every input-gradient (the forward kernel called from backward) and weight-gradient call"""
+
+    def __init__(self, U):
+        import torch
+        self.U, self.phase, self.calls = U, "forward", []
+        gemm, wgrad = U.gather_gemm, U.gather_gemm_wgrad
+
+        def timed(kind, fn, shape):
+            def run(*a, **k):
+                if self.phase != "backward":
+                    return fn(*a, **k)
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                out = fn(*a, **k)
+                e1.record()
+                self.calls.append((kind, e0, e1, shape(*a)))
+                return out
+            return run
+        U.gather_gemm = timed("dgrad", gemm, lambda x, idx, *r: None)
+        U.gather_gemm_wgrad = timed("wgrad", wgrad, lambda x, idx, g, *r: (idx, x.shape[1], g.shape[1]))
+
+    def summary(self):
+        out = {"dgrad": 0.0, "wgrad": 0.0}
+        for kind, e0, e1, _ in self.calls:
+            out[kind] += e0.elapsed_time(e1)
+        return out
+
+    def wgrad_rates(self):
+        """per (c_in, c_out): ms, TFLOP/s (2 nnz_taps c_in c_out) and GB/s (gathered x rows, g read once per tap with a
+        source, the table, dW) of the weight-gradient kernel in the recorded step"""
+        per = {}
+        for kind, e0, e1, shp in self.calls:
+            if kind != "wgrad":
+                continue
+            idx, ci, co = shp
+            nnz = int((idx >= 0).sum())
+            n_out, K = idx.shape
+            r = per.setdefault(f"{ci}x{co}", dict(ms=0.0, flop=0.0, bytes=0.0, calls=0))
+            r["ms"] += e0.elapsed_time(e1)
+            r["flop"] += 2.0 * nnz * ci * co
+            r["bytes"] += 4.0 * (nnz * ci + nnz * co + n_out * K + K * ci * co)
+            r["calls"] += 1
+        return {k: dict(ms=round(v["ms"], 3), calls=v["calls"], tflops=round(v["flop"] / v["ms"] / 1e9, 2),
+                        gbs=round(v["bytes"] / v["ms"] / 1e6, 1)) for k, v in per.items()}
+
+
+def main(argv=None):
+    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
+    ap.add_argument("--scene", choices=("sphere", "cfg4"), default="sphere")
+    ap.add_argument("--points", type=int, default=200_000)
+    ap.add_argument("--depth", type=int, default=4)
+    ap.add_argument("--precision", choices=("fp32", "tf32", "tc"), default="fp32")
+    ap.add_argument("--steps", type=int, default=30)
+    ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--out", default=None, help="checkpoint path ({'state_dict': ...})")
+    args = ap.parse_args(argv)
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    import torch
+    if not torch.cuda.is_available():
+        raise SystemExit("train_unet.py needs a CUDA device")
+    import nksr_b200.unet as U
+    from bench import gpu_info
+    from nksr_b200 import training as T
+    from nksr_b200.network import NKSRNetwork
+    torch.use_deterministic_algorithms(True, warn_only=True)
+    dev = torch.device("cuda:0")
+    scene = make_scene(args.scene, args.points, args.depth, dev)
+    net = NKSRNetwork(dict(backbone="unet", tree_depth=args.depth, kernel_dim=4, precision=args.precision,
+                           trainable=True, seed=args.seed)).to(dev)
+    opt = T.make_optimizer(net)
+    gen = torch.Generator(device=dev).manual_seed(args.seed)
+    timer = KernelTimer(U)
+    info = dict(gpu_info(0), scene=args.scene, points=int(scene.xyz.shape[0]), voxel_size=scene.voxel_size,
+                depth=args.depth, precision=args.precision,
+                voxels=[scene.enc_svh.num_voxels(l) for l in range(args.depth)])
+    print(json.dumps(dict(setup=info)), flush=True)
+    rows = []
+    for step in range(args.steps):
+        timer.calls.clear()
+        ev = {"start": torch.cuda.Event(enable_timing=True)}
+        ev["start"].record()
+
+        def marks(name):
+            ev[name] = torch.cuda.Event(enable_timing=True)
+            ev[name].record()
+            timer.phase = {"forward": "backward", "backward": "step"}.get(name, "forward")
+        timer.phase = "forward"
+        l_struct, l_udf = T.train_step(net, opt, scene, gen, marks)
+        timer.phase = "forward"
+        torch.cuda.synchronize()
+        k = timer.summary()
+        row = dict(step=step, structure=round(float(l_struct), 6), udf=round(float(l_udf), 6),
+                   forward_ms=round(ev["start"].elapsed_time(ev["forward"]), 3),
+                   backward_ms=round(ev["forward"].elapsed_time(ev["backward"]), 3),
+                   dgrad_ms=round(k["dgrad"], 3), wgrad_ms=round(k["wgrad"], 3),
+                   step_ms=round(ev["backward"].elapsed_time(ev["step"]), 3))
+        rows.append(row)
+        print(json.dumps(row), flush=True)
+    timed = rows[2:] if len(rows) > 2 else rows
+    med = {key: round(statistics.median(r[key] for r in timed), 3)
+           for key in ("forward_ms", "backward_ms", "dgrad_ms", "wgrad_ms", "step_ms")}
+    med["backward_over_forward"] = round(med["backward_ms"] / med["forward_ms"], 3)
+    print(json.dumps(dict(summary=med, wgrad_last_step=timer.wgrad_rates(), **info)), flush=True)
+    if args.out:
+        torch.save({"state_dict": net.state_dict()}, args.out)
+
+
+if __name__ == "__main__":
+    main()
