@@ -412,7 +412,11 @@ int nksr_spmv_stream(const int64_t* rowptr, const int32_t* col, const float* val
     return NKSR_E_INVALID;
   if (plan_bytes < spmv_plan_bytes(nnz)) return NKSR_E_WORKSPACE;
   cudaStream_t s = as_stream(stream);
-  if (cudaMemsetAsync(y, 0, (size_t)n * sizeof(float), s) != cudaSuccess) return NKSR_E_CUDA;   // empty rows
+  // the streamed part writes every row of [0, split_row), empty ones included; when those rows hold no entry at all,
+  // nothing is streamed and they are zeroed here
+  if (split_row > 0 && split_nnz == 0 &&
+      cudaMemsetAsync(y, 0, (size_t)split_row * sizeof(float), s) != cudaSuccess)
+    return NKSR_E_CUDA;
   if (split_row > 0 && split_nnz > 0) {
     SpmvPlan plan = spmv_plan_carve(plan_buf, split_row, split_nnz);
     if (spmv_stream_prepare() != NKSR_OK) return NKSR_E_CUDA;

@@ -68,12 +68,14 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, unsigned by
                : "memory");
 }
 
-// first_row[t] = row that contains entry t * kTile (last row whose start is <= that entry); first_row[ntiles] = n
+// first_row[t] = row that contains entry t * kTile (last row whose start is <= that entry); first_row[0] = 0, so that
+// tile 0 also writes the empty rows the matrix may start with; first_row[ntiles] = n
 __global__ void k_spmv_plan(const int64_t* __restrict__ rowptr, int64_t n, int64_t ntiles,
                             int32_t* __restrict__ first_row) {
   const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (t > ntiles) return;
   if (t == ntiles) { first_row[t] = (int32_t)n; return; }
+  if (t == 0) { first_row[0] = 0; return; }
   const int64_t e = t * kTile;
   int64_t lo = 0, hi = n;   // first row with rowptr[row] > e
   while (lo < hi) {
@@ -166,8 +168,11 @@ k_spmv_stream(const int64_t* __restrict__ rowptr, const int32_t* __restrict__ co
     const int64_t rlast = first_row[t + 1] < n ? first_row[t + 1] : n - 1;   // last row the slice describes
     for (int64_t row = r0 + wid; row <= rlast; row += kStreamWarps) {
       const int64_t b = rp[row - ra];
-      if (b >= e1) break;
       const int64_t e = rp[row - ra + 1];
+      // an empty row that starts exactly at the tile's end belongs to no later tile (first_row[t + 1] is the last
+      // row starting there): this tile writes its zero.  With first_row[0] = 0 for the rows before entry 0, every
+      // row of [0, n) is written
+      if (b > e1 || (b == e1 && e > b)) break;
       const int lo = (int)((b > e0 ? b : e0) - e0), hi = (int)((e < e1 ? e : e1) - e0);
       float acc = 0.f;
       for (int p = lo + lane; p < hi; p += 32) acc += st.val[p];

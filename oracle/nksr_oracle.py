@@ -384,12 +384,19 @@ def structural_pattern(svh: OracleSVH):
 
 
 # --------------------------------------------------------------------------- solver
-def pcg(A, b, tol=1e-5, max_iter=2000, x0=None, dtype=np.float64):
-    """Jacobi-preconditioned CG (SPEC S7); stop at ||r|| <= tol*||b||.  Returns x, iters, relres."""
+def _jacobi_inverse(A, diag, dtype):
+    """1/d where d > 0, else 0 (the solver's preconditioner); d = A's diagonal unless given"""
+    d = A.diagonal() if diag is None else np.asarray(diag, np.float64)
+    return np.where(d > 0, 1.0 / np.where(d > 0, d, 1), 0.0).astype(dtype)
+
+
+def pcg(A, b, tol=1e-5, max_iter=2000, x0=None, dtype=np.float64, diag=None, history=None):
+    """Jacobi-preconditioned CG (SPEC S7); stop at ||r|| <= tol*||b||.  Returns x, iters, relres.
+    diag: the preconditioner's diagonal (default: A's).  history: a list that receives (x_k, relres_k) after every
+    iteration k = 1, 2, ..."""
     A = A.astype(dtype)
     b = b.astype(dtype)
-    d = A.diagonal()
-    dinv = np.where(d > 0, 1.0 / np.where(d > 0, d, 1), 0.0).astype(dtype)
+    dinv = _jacobi_inverse(A, diag, dtype)
     x = np.zeros_like(b) if x0 is None else x0.astype(dtype).copy()
     r = b - A @ x
     z = dinv * r
@@ -413,7 +420,47 @@ def pcg(A, b, tol=1e-5, max_iter=2000, x0=None, dtype=np.float64):
         p = z + beta * p
         it += 1
         res = float(np.linalg.norm(r.astype(np.float64))) / bn
+        if history is not None:
+            history.append((x.copy(), res))
     return x, it, res
+
+
+def pcg_cg(A, b, tol=1e-5, max_iter=2000, dtype=np.float64, diag=None, history=None):
+    """The same Jacobi-PCG in the Chronopoulos-Gear arrangement of the distributed solve (csrc/solve.cu, nksr_dcg_*):
+    one sweep per iteration forms w = A u and the three dots (r,u), (w,u), (r,r) of the CURRENT iterate, then
+        beta = gamma / gamma_prev,  alpha = gamma / (delta - beta gamma / alpha_prev)   (alpha = gamma / delta first)
+        p = u + beta p;  s = w + beta s;  x += alpha p;  r -= alpha s;  u = M^-1 r.
+    In exact arithmetic its iterates are those of pcg().  Returns x, iters, relres; history as in pcg()."""
+    A = A.astype(dtype)
+    b = b.astype(dtype)
+    dinv = _jacobi_inverse(A, diag, dtype)
+    x = np.zeros_like(b)
+    r = b.copy()
+    u = dinv * r
+    p = np.zeros_like(b)
+    s = np.zeros_like(b)
+    bn = float(np.linalg.norm(b.astype(np.float64)))
+    if bn == 0:
+        return x, 0, 0.0
+    it, gamma_prev, alpha_prev = 0, 0.0, 0.0
+    while True:
+        w = A @ u
+        gamma = float(r.astype(np.float64) @ u.astype(np.float64))
+        delta = float(w.astype(np.float64) @ u.astype(np.float64))
+        res = float(np.linalg.norm(r.astype(np.float64))) / bn
+        if res <= tol or it >= max_iter:
+            return x, it, res
+        beta = gamma / gamma_prev if it > 0 else 0.0
+        alpha = gamma / (delta - beta * gamma / alpha_prev) if it > 0 else gamma / delta
+        p = u + dtype(beta) * p
+        s = w + dtype(beta) * s
+        x += dtype(alpha) * p
+        r -= dtype(alpha) * s
+        u = dinv * r
+        it += 1
+        gamma_prev, alpha_prev = gamma, alpha
+        if history is not None:
+            history.append((x.copy(), float(np.linalg.norm(r.astype(np.float64))) / bn))
 
 
 # --------------------------------------------------------------------------- field evaluation

@@ -29,6 +29,24 @@ KAPPA_GEMM_TF32 = 256.0
 # (2^13 u), plus the accumulation.  Worst 9133 (wgmma).
 KAPPA_GEMM_TF32_OPERANDS = 2.0 ** 15
 
+# solve.cu / spmv_stream.cuh: one SpMV (row and streamed kernels) against the scale |A| |x|.  Worst 2.89 (streamed,
+# random-graph Laplacian, rows up to ~7000 entries).
+KAPPA_SPMV = 16.0
+# solve.cu, Jacobi-PCG against fp64 PCG on the same fp32 matrix (tests/test_gpu_solver.py).  First iterate
+# x_1 = alpha_0 D^-1 b entry by entry, scale |x_1| (1 + |p|^T |A| |p| / p^T A p).  Worst 1.05 (100^3 Laplacian).
+KAPPA_PCG_X1 = 8.0
+# Iterate k, normwise: ||x_k - x_k^ref|| <= kappa k u ||x_k^ref||, k = 1 ... 20.  Worst 0.997 (100^3 Laplacian).
+KAPPA_PCG_ITER = 7.0
+# Reported relative residual info[1] after k iterations against the reference's recursive residual r_k:
+# |info[1] - ||r_k|| / ||b||| <= kappa k u ||r_k|| / ||b||.  Worst 0.97 (Chronopoulos-Gear, shapenet); PCG 0.79.
+KAPPA_PCG_RES = 6.0
+# True fp64 residual of the returned x <= 2 reported + kappa floor, floor = u (|| |A| |x| || + ||b||) / ||b||, for
+# tol 1e-3 ... 1e-7.  Worst 1.01 (Chronopoulos-Gear, sphere); PCG 0.93.
+KAPPA_PCG_FLOOR = 8.0
+# Chronopoulos-Gear kernels (nksr_dcg_*), iterate k normwise against fp64 PCG, and R ranks against one rank.  Worst
+# 1.31 (sphere, 2 and 3 ranks, local subsystems).
+KAPPA_DCG_ITER = 8.0
+
 
 def _union(*mats):
     """rows, cols and the values of each sparse matrix on the union of their stored patterns"""

@@ -75,6 +75,34 @@ def test_pcg_matches_dense_solve_and_field_vanishes_on_points():
     assert np.mean(np.sum(-g * outward, axis=1)) > 0.8       # grad f = -normal
 
 
+def test_chronopoulos_gear_reference_has_the_pcg_iterates():
+    """oracle.pcg_cg (the distributed solve's arrangement) against oracle.pcg, both fp64, on the fp32 values of the
+    sphere system of the GPU solver tests (4000 points, W 0.05, 3 levels): the first 20 iterates and residuals agree to
+    1e-10 relative.  At tol 1e-6 (about 165 iterations, long after orthogonality is lost) the two stop within 3
+    iterations of each other (164 and 166)."""
+    xyz, _ = clouds.sphere(4000)
+    W = 0.05
+    svh = O.OracleSVH(W, 3).build_point_splatting(xyz)
+    rng = np.random.default_rng(11)
+    feats = [(0.5 + 0.2 * rng.normal(size=(svh.n(l), 4))).astype(np.float32) for l in range(3)]
+    nxyz = np.concatenate([svh.centers(0), svh.centers(1)])
+    rng = np.random.default_rng(3)
+    nval = rng.normal(size=nxyz.shape).astype(np.float32)
+    nval /= np.linalg.norm(nval, axis=1, keepdims=True)
+    A, b, _ = O.build_system(svh, feats, xyz, nxyz, nval, 1e4 / xyz.shape[0], 1e4 / nxyz.shape[0] * W * W, 1.0)
+    A32, b32 = A.astype(np.float32).astype(np.float64), b.astype(np.float32).astype(np.float64)
+    h_pcg, h_cg = [], []
+    O.pcg(A32, b32, 0.0, 20, history=h_pcg)
+    O.pcg_cg(A32, b32, 0.0, 20, history=h_cg)
+    assert len(h_pcg) == len(h_cg) == 20
+    for k, ((x1, r1), (x2, r2)) in enumerate(zip(h_pcg, h_cg), 1):
+        assert np.linalg.norm(x1 - x2) <= 1e-10 * np.linalg.norm(x1), k
+        assert abs(r1 - r2) <= 1e-10 * r1, k
+    _, it1, res1 = O.pcg(A32, b32, 1e-6, 5000)
+    _, it2, res2 = O.pcg_cg(A32, b32, 1e-6, 5000)
+    assert abs(it1 - it2) <= 3 and res1 <= 1e-6 and res2 <= 1e-6
+
+
 def test_gradient_matches_finite_differences():
     svh, feats, xyz, A, b = _small_system()
     x, _, _ = O.pcg(A, b, 1e-8, 3000)

@@ -8,7 +8,7 @@ import torch
 
 from oracle import nksr_oracle as O
 from tests import clouds
-from tests.bounds import (KAPPA_FIELD, KAPPA_GRAM, KAPPA_RHS, KAPPA_ROWS, assert_within, level_of,
+from tests.bounds import (KAPPA_FIELD, KAPPA_GRAM, KAPPA_RHS, KAPPA_ROWS, KAPPA_SPMV, assert_within, level_of,
                           level_pair_label)
 
 pytestmark = pytest.mark.gpu
@@ -378,7 +378,7 @@ def test_spmv_and_pcg_match_oracle(cuda):
     y = torch.empty_like(x)
     L.call("nksr_spmv", s.rowptr, s.col, s.val, x, y, A.shape[0], L.stream_ptr(cuda))
     yr = A @ _np(x).astype(np.float64)
-    assert np.abs(_np(y) - yr).max() <= 1e-5 * np.abs(yr).max()
+    assert_within(_np(y), yr, abs(A) @ np.abs(_np(x)).astype(np.float64), KAPPA_SPMV, "row SpMV (assembled)")
     # PCG: converged, and the solution solves the oracle's system
     assert field.solve_info["relative_residual"] <= 1e-6
     A_ref, b_ref, _ = O.build_system(osvh, feats, xyz, nxyz, nval, pw, nw, rw)
@@ -452,9 +452,9 @@ def test_streamed_spmv_matches_row_spmv(cuda, kind):
     A = sp.csr_matrix((_np(val).astype(np.float64), _np(col), _np(rowptr)), shape=(n, n))
     ref = A @ _np(x).astype(np.float64)
     absA = abs(A) @ np.abs(_np(x)).astype(np.float64)           # scale of the terms of each row sum
-    assert np.all(np.abs(ys[0] - ref) <= 2e-6 * absA + 1e-30)
-    assert np.all(np.abs(ys[1] - ref) <= 2e-6 * absA + 1e-30)
-    assert np.all(np.abs(_np(y_rows) - ref) <= 2e-6 * absA + 1e-30)
+    assert_within(ys[0], ref, absA, KAPPA_SPMV, f"streamed SpMV ({kind})")
+    assert_within(ys[1], ref, absA, KAPPA_SPMV, f"streamed SpMV, last third by rows ({kind})")
+    assert_within(_np(y_rows), ref, absA, KAPPA_SPMV, f"row SpMV ({kind})")
 
 
 def test_streamed_pcg_is_the_row_pcg(cuda):
