@@ -203,6 +203,21 @@ NKSR_API int nksr_gram_place(const nksr_svh_t* svh, int l, int k, int32_t* rank8
 NKSR_API int nksr_gram_fill_placed(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
                           const int32_t* cnt, const int64_t* rowptr, const nksr_placement_t* placement,
                           int32_t* col, float* val, float* rhs, float* diag, void* stream);
+/* nksr_gram_fill_placed on the rows [row_begin, row_end) only (row_end = -1: to the last row) */
+NKSR_API int nksr_gram_fill_placed_rows(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
+                               const int32_t* cnt, const int64_t* rowptr, const nksr_placement_t* placement,
+                               int64_t row_begin, int64_t row_end, int32_t* col, float* val, float* rhs,
+                               float* diag, void* stream);
+/* the same matrix with the brick fill: the rows of a level below c->split_level that holds at least
+ * min_locations_per_voxel constraint locations (positions + normals) per voxel are filled one brick (the level-l voxels
+ * under one level-(l+2) key) per block, every constraint line of a source voxel loaded once per brick and multiplied
+ * into all its target rows there; every other row runs nksr_gram_fill_placed.  Same CSR pattern and storage order; the
+ * 27 per-source partial sums of a bricked row are added in a different (fixed) order.  Compact gradient rows and
+ * depth > 4 run nksr_gram_fill_placed on every row. */
+NKSR_API int nksr_gram_fill_brick(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
+                         const int32_t* cnt, const int64_t* rowptr, const nksr_placement_t* placement,
+                         int32_t* col, float* val, float* rhs, float* diag, float min_locations_per_voxel,
+                         void* stream);
 
 /* the same fill with the sibling-group decomposition (one warp per level-(l+1) voxel = up to eight matrix rows
  * that share their constraint rows, column tables and flush indices): same CSR, same order.  Needs depth <= 4

@@ -81,6 +81,8 @@ _SIGNATURES = {
     "nksr_gram_count_own": ("i", "Spp"),
     "nksr_gram_place": ("i", "Siipppp" + "p"),
     "nksr_gram_fill_placed": ("i", "SFKppPppppp"),
+    "nksr_gram_fill_placed_rows": ("i", "SFKppPqqppppp"),
+    "nksr_gram_fill_brick": ("i", "SFKppPppppfp"),
     "nksr_gram_fill_grouped": ("i", "SFKppPppppp"),
     "nksr_gram_count_grouped": ("i", "Spp"),
     "nksr_nbr125_search": ("i", "pqpp"),

@@ -275,7 +275,7 @@ k_gram_blocks(nksr_svh_t svh, nksr_constraints_t cs, float* __restrict__ mblocks
 // bitwise the one of the plain layout.
 template <bool COMPACT, int MAXL, int MINB, bool PLACED, bool ILV>
 __global__ void __launch_bounds__(kWarps * 32, MINB)
-k_gram_fill(nksr_svh_t svh, nksr_feat_t feat, nksr_constraints_t cs, int64_t n_total,
+k_gram_fill(nksr_svh_t svh, nksr_feat_t feat, nksr_constraints_t cs, int64_t row_begin, int64_t row_end,
             const int32_t* __restrict__ cnt, const int64_t* __restrict__ rowptr, int32_t* __restrict__ col_out,
             float* __restrict__ val_out, float* __restrict__ rhs, float* __restrict__ diag,
             int32_t* __restrict__ cursor, const PlaceArg<PLACED> place) {
@@ -284,8 +284,8 @@ k_gram_fill(nksr_svh_t svh, nksr_feat_t feat, nksr_constraints_t cs, int64_t n_t
   const int wid = threadIdx.x >> 5;
   // coarse rows own thousands of constraint rows, fine rows a few dozen: schedule the heavy
   // (coarse, high index) rows first so that the tail of the grid is made of light rows
-  const int64_t row = n_total - 1 - (blockIdx.x * (int64_t)kWarps + wid);
-  if (row < 0) return;
+  const int64_t row = row_end - 1 - (blockIdx.x * (int64_t)kWarps + wid);
+  if (row < row_begin) return;
   int l, i;
   row_of_warp(svh, row, l, i);
   const int L = svh.depth;
@@ -481,68 +481,9 @@ k_gram_fill(nksr_svh_t svh, nksr_feat_t feat, nksr_constraints_t cs, int64_t n_t
     }
     __syncwarp();
   }
-  // regulariser: R_{i,i+d} = w_reg * B3(d) * <z_i, z_{i+d}>  (SPEC S5)
-  if (cs.w_reg != 0.f && my_u >= 0) {
-    const int C = feat.channels;
-    const float* zi = feat.z[l] + (int64_t)i * C;
-    const float* zn = feat.z[l] + (int64_t)my_u * C;
-    float d = 0.f;
-    for (int c = 0; c < C; ++c) d = fmaf(__ldg(zi + c), __ldg(zn + c), d);
-    const float bw = (ldx == 0 ? 0.75f : 0.125f) * (ldy == 0 ? 0.75f : 0.125f) * (ldz == 0 ? 0.75f : 0.125f);
-    acc[(ldx + 2) * 25 + (ldy + 2) * 5 + (ldz + 2)] += cs.w_reg * bw * d;
-  }
+  gram_row_regulariser(feat, cs, l, i, my_u, lane, acc);
   __syncwarp();
-  // write-out in structural order: the 125 same-level slots (4 chunks of 32), then the 64 slots of every coarser level
-  // (2 chunks each) -- the level offset k is uniform inside a chunk, so the box bounds, the ancestor and its parent are
-  // computed once per level instead of once per slot (in the first version a chunk could straddle two levels)
-  const int64_t p0 = rowptr[row];
-  int written = 0;
-  auto emit = [&](const int c, const int k, const int t, const int ds, const int sm) {
-    const unsigned m = __ballot_sync(0xffffffffu, c >= 0);
-    if (c >= 0) {
-      const int64_t p = p0 + written + __popc(m & ((1u << lane) - 1u));
-      const float v = acc[t];
-      const int64_t gc = svh.offset[l + k] + c;
-      col_out[p] = (int32_t)gc;
-      val_out[p] = v;
-      if (k == 0 && c == i) diag[row] = v;
-      if (k > 0) {  // transposed copy into the coarse row's finer-level segment
-        const int64_t q = rowptr[gc] + cnt[gc] +
-                          (PLACED ? place.pos(l, k, c, ds, i, sm) : atomicAdd(cursor + gc, 1));
-        col_out[q] = (int32_t)row;
-        val_out[q] = v;
-      }
-    }
-    written += __popc(m);
-  };
-  for (int t0 = 0; t0 < 125; t0 += 32) {
-    const int t = t0 + lane;
-    int k = 0;
-    const int c = t < 125 ? slot_column(svh, l, g, t, k) : -1;
-    emit(c, 0, t, 0, 0);
-  }
-#pragma unroll
-  for (int k = 1; k < MAXL; ++k) {
-    if (k <= nup) {
-      const int lox = ((g.ux - 1) >> k) - 1, loy = ((g.uy - 1) >> k) - 1, loz = ((g.uz - 1) >> k) - 1;
-      const int hix = ((g.ux + 1) >> k) + 1, hiy = ((g.uy + 1) >> k) + 1, hiz = ((g.uz + 1) >> k) + 1;
-      const int ax = g.ux >> k, ay = g.uy >> k, az = g.uz >> k;
-      const int a = g.anc[k];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int q = h * 32 + lane;
-        const int cx = lox + (q >> 4), cy = loy + ((q >> 2) & 3), cz = loz + (q & 3);
-        int c = -1, ds = 0, sm = 0;
-        if (a >= 0 && cx <= hix && cy <= hiy && cz <= hiz) {
-          c = lookup_near(svh, l + k, a, ax, ay, az, cx, cy, cz);
-          const int dx = cx - ax, dy = cy - ay, dz = cz - az;
-          ds = (dx + 2) * 25 + (dy + 2) * 5 + (dz + 2);
-          sm = ((dx == -2 || dx == 2) ? 4 : 0) | ((dy == -2 || dy == 2) ? 2 : 0) | ((dz == -2 || dz == 2) ? 1 : 0);
-        }
-        emit(c, k, 125 + 64 * (k - 1) + q, ds, sm);
-      }
-    }
-  }
+  gram_row_writeout<MAXL, PLACED>(svh, l, i, row, g, acc, cnt, rowptr, col_out, val_out, diag, cursor, place, lane);
   if (lane == 0) rhs[row] = bsum;
 }
 
@@ -754,17 +695,19 @@ namespace {
 template <bool PLACED>
 int launch_fill(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c, const int32_t* cnt,
                 const int64_t* rowptr, int32_t* col, float* val, float* rhs, float* diag, int32_t* cursor,
-                const PlaceArg<PLACED>& place, void* stream) {
+                const PlaceArg<PLACED>& place, int64_t row_begin, int64_t row_end, void* stream) {
   if (!svh || !feat || !c || svh->depth < 1 || svh->depth > NKSR_MAX_DEPTH) return NKSR_E_INVALID;
   if (!svh->nbr125_top && !svh->parent[svh->depth - 1]) return NKSR_E_INVALID;
   const int64_t n = total_unknowns(svh);
-  if (n == 0) return NKSR_OK;
+  if (row_end < 0) row_end = n;
+  if (row_begin < 0 || row_begin > row_end || row_end > n) return NKSR_E_INVALID;
+  if (row_begin == row_end) return NKSR_OK;
   cudaStream_t s = as_stream(stream);
   const size_t smem = (size_t)kWarps * kMaxSlots * sizeof(float);
-  const int grid = grid_for(n, kWarps);
+  const int grid = grid_for(row_end - row_begin, kWarps);
 #define NKSR_FILL(COMPACT, MAXL, MINB, ILV)                                                                  \
-  k_gram_fill<COMPACT, MAXL, MINB, PLACED, ILV><<<grid, kWarps * 32, smem, s>>>(*svh, *feat, *c, n, cnt, rowptr, col, \
-                                                                                val, rhs, diag, cursor, place)
+  k_gram_fill<COMPACT, MAXL, MINB, PLACED, ILV><<<grid, kWarps * 32, smem, s>>>(                             \
+      *svh, *feat, *c, row_begin, row_end, cnt, rowptr, col, val, rhs, diag, cursor, place)
   // 4 resident blocks per SM (64 registers) for depth <= 4; 5 blocks (48 registers) was measured
   // 1.7x slower (register starvation cuts the loads in flight per warp)
   if (c->nrm_compact == 2) {                          // interleaved rows
@@ -787,16 +730,23 @@ int nksr_gram_fill(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_co
                    const int64_t* rowptr, int32_t* col, float* val, float* rhs, float* diag, int32_t* cursor,
                    void* stream) {
   if (!cursor) return NKSR_E_INVALID;
-  return launch_fill<false>(svh, feat, c, cnt, rowptr, col, val, rhs, diag, cursor, PlaceArg<false>{}, stream);
+  return launch_fill<false>(svh, feat, c, cnt, rowptr, col, val, rhs, diag, cursor, PlaceArg<false>{}, 0, -1, stream);
 }
 
 int nksr_gram_fill_placed(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
                           const int32_t* cnt, const int64_t* rowptr, const nksr_placement_t* placement,
                           int32_t* col, float* val, float* rhs, float* diag, void* stream) {
+  return nksr_gram_fill_placed_rows(svh, feat, c, cnt, rowptr, placement, 0, -1, col, val, rhs, diag, stream);
+}
+
+int nksr_gram_fill_placed_rows(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
+                               const int32_t* cnt, const int64_t* rowptr, const nksr_placement_t* placement,
+                               int64_t row_begin, int64_t row_end, int32_t* col, float* val, float* rhs, float* diag,
+                               void* stream) {
   if (!placement) return NKSR_E_INVALID;
   PlaceArg<true> place;
   place.t = *placement;
-  return launch_fill<true>(svh, feat, c, cnt, rowptr, col, val, rhs, diag, nullptr, place, stream);
+  return launch_fill<true>(svh, feat, c, cnt, rowptr, col, val, rhs, diag, nullptr, place, row_begin, row_end, stream);
 }
 
 int nksr_gram_sort_down(const int32_t* cnt, const int32_t* cnt_down, const int64_t* rowptr, const int32_t* rows,

@@ -107,4 +107,81 @@ __device__ __forceinline__ void row_of_warp(const nksr_svh_t& svh, int64_t row, 
   i = (int)(row - svh.offset[l]);
 }
 
+// regulariser R_{i,i+d} = w_reg * B3(d) * <z_i, z_{i+d}> (SPEC S5) added to the row's tile; lane s < 27 owns offset d(s),
+// my_u = nbr27[l][i][s] (-1 for the other lanes)
+__device__ __forceinline__ void gram_row_regulariser(const nksr_feat_t& feat, const nksr_constraints_t& cs, int l, int i,
+                                                     int my_u, int lane, float* __restrict__ acc) {
+  if (cs.w_reg == 0.f || my_u < 0) return;
+  const int sl = lane < 27 ? lane : 13;
+  const int ldx = c_d27[sl][0], ldy = c_d27[sl][1], ldz = c_d27[sl][2];
+  const int C = feat.channels;
+  const float* zi = feat.z[l] + (int64_t)i * C;
+  const float* zn = feat.z[l] + (int64_t)my_u * C;
+  float d = 0.f;
+  for (int c = 0; c < C; ++c) d = fmaf(__ldg(zi + c), __ldg(zn + c), d);
+  const float bw = (ldx == 0 ? 0.75f : 0.125f) * (ldy == 0 ? 0.75f : 0.125f) * (ldz == 0 ? 0.75f : 0.125f);
+  acc[(ldx + 2) * 25 + (ldy + 2) * 5 + (ldz + 2)] += cs.w_reg * bw * d;
+}
+
+// write-out of row (l,i) from its tile `acc` (indexed by structural slot) in structural order: the 125 same-level slots
+// (4 chunks of 32), then the 64 slots of every coarser level (2 chunks each) -- the level offset is uniform inside a chunk,
+// so the box bounds, the ancestor and its parent are computed once per level (in the first version a chunk could
+// straddle two levels).  Coarser-level entries also go, transposed, to the coarse row's finer-level segment.
+template <int MAXL, bool PLACED>
+__device__ __forceinline__ void gram_row_writeout(const nksr_svh_t& svh, int l, int i, int64_t row, const RowGeom& g,
+                                                  const float* __restrict__ acc, const int32_t* __restrict__ cnt,
+                                                  const int64_t* __restrict__ rowptr, int32_t* __restrict__ col_out,
+                                                  float* __restrict__ val_out, float* __restrict__ diag,
+                                                  int32_t* __restrict__ cursor, const PlaceArg<PLACED>& place, int lane) {
+  const int nup = svh.depth - 1 - l;
+  const int64_t p0 = rowptr[row];
+  int written = 0;
+  auto emit = [&](const int c, const int k, const int t, const int ds, const int sm) {
+    const unsigned m = __ballot_sync(0xffffffffu, c >= 0);
+    if (c >= 0) {
+      const int64_t p = p0 + written + __popc(m & ((1u << lane) - 1u));
+      const float v = acc[t];
+      const int64_t gc = svh.offset[l + k] + c;
+      col_out[p] = (int32_t)gc;
+      val_out[p] = v;
+      if (k == 0 && c == i) diag[row] = v;
+      if (k > 0) {  // transposed copy into the coarse row's finer-level segment
+        const int64_t q = rowptr[gc] + cnt[gc] +
+                          (PLACED ? place.pos(l, k, c, ds, i, sm) : atomicAdd(cursor + gc, 1));
+        col_out[q] = (int32_t)row;
+        val_out[q] = v;
+      }
+    }
+    written += __popc(m);
+  };
+  for (int t0 = 0; t0 < 125; t0 += 32) {
+    const int t = t0 + lane;
+    int k = 0;
+    const int c = t < 125 ? slot_column(svh, l, g, t, k) : -1;
+    emit(c, 0, t, 0, 0);
+  }
+#pragma unroll
+  for (int k = 1; k < MAXL; ++k) {
+    if (k <= nup) {
+      const int lox = ((g.ux - 1) >> k) - 1, loy = ((g.uy - 1) >> k) - 1, loz = ((g.uz - 1) >> k) - 1;
+      const int hix = ((g.ux + 1) >> k) + 1, hiy = ((g.uy + 1) >> k) + 1, hiz = ((g.uz + 1) >> k) + 1;
+      const int ax = g.ux >> k, ay = g.uy >> k, az = g.uz >> k;
+      const int a = g.anc[k];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int q = h * 32 + lane;
+        const int cx = lox + (q >> 4), cy = loy + ((q >> 2) & 3), cz = loz + (q & 3);
+        int c = -1, ds = 0, sm = 0;
+        if (a >= 0 && cx <= hix && cy <= hiy && cz <= hiz) {
+          c = lookup_near(svh, l + k, a, ax, ay, az, cx, cy, cz);
+          const int dx = cx - ax, dy = cy - ay, dz = cz - az;
+          ds = (dx + 2) * 25 + (dy + 2) * 5 + (dz + 2);
+          sm = ((dx == -2 || dx == 2) ? 4 : 0) | ((dy == -2 || dy == 2) ? 2 : 0) | ((dz == -2 || dz == 2) ? 1 : 0);
+        }
+        emit(c, k, 125 + 64 * (k - 1) + q, ds, sm);
+      }
+    }
+  }
+}
+
 }  // namespace

@@ -32,6 +32,11 @@ from .svh import SparseFeatureHierarchy
 DEFAULT_PLACEMENT = "structural"
 # the layout every parity test runs on unless a test selects the other
 DEFAULT_ROW_LAYOUT = "levels"
+# the Gram fill (solver_config['fill'] or the NKSR_FILL environment variable override it): "brick", "rows", "grouped"
+DEFAULT_FILL = "brick"
+# 'brick' bricks a fine level only when it holds at least this many constraint locations per voxel (measured on H100:
+# faster at 18 per voxel, slower at 1.7 and 4.9; DESIGN 4.1)
+BRICK_MIN_LOCATIONS_PER_VOXEL = 8.0
 
 
 _TOTAL_MEMORY = {}
@@ -327,7 +332,7 @@ class KernelField(BaseField):
         if compact is None:
             compact = os.environ.get("NKSR_COMPACT_ROWS", "0") == "1"
         ilv = (layout == "interleaved" and svh.depth <= 4 and not (self.approx_kernel_grad and compact)
-               and (self.solver_config.get("fill") or os.environ.get("NKSR_FILL") or "rows") == "rows"
+               and (self.solver_config.get("fill") or os.environ.get("NKSR_FILL") or DEFAULT_FILL) in ("rows", "brick")
                and (self.solver_config.get("rows") or os.environ.get("NKSR_ROWS") or "location") == "location")
         _, _, _, range_pos, e_pos = self._sorted_rows(pos_xyz, 0, interleaved=ilv)
         keep += [range_pos, e_pos]
@@ -392,15 +397,20 @@ class KernelField(BaseField):
         val = torch.empty(nnz + 4, dtype=torch.float32, device=dev)[:nnz]
         rhs = torch.empty(n, dtype=torch.float32, device=dev)
         diag = torch.zeros(n, dtype=torch.float32, device=dev)
-        # numeric phase.  'rows' (default): one warp per matrix row (csrc/assemble.cu); 'grouped': one warp per
+        # numeric phase.  'brick' (default): the rows of the dense levels below the block split level one brick of
+        # 4^3 rows per block, every constraint line of a source voxel loaded once per brick (csrc/gram_fill_brick.cu),
+        # the other rows as 'rows'; 'rows': one warp per matrix row (csrc/assemble.cu); 'grouped': one warp per
         # sibling group -- eight rows share their constraint lines, column tables and flush indices
         # (csrc/gram_fill_group.cu).  The sharing halves the loads but the per-sibling tests and flushes cost as many
         # instructions as they save, and 13.4 KB of shared memory + 128 registers per warp cut the resident warps per SM
-        fill = self.solver_config.get("fill") or os.environ.get("NKSR_FILL") or "rows"
-        if fill not in ("grouped", "rows"):
-            raise ValueError("solver_config['fill'] must be 'grouped' or 'rows'")
+        fill = self.solver_config.get("fill") or os.environ.get("NKSR_FILL") or DEFAULT_FILL
+        if fill not in ("brick", "grouped", "rows"):
+            raise ValueError("solver_config['fill'] must be 'brick', 'grouped' or 'rows'")
         if place is not None and fill == "grouped" and svh.depth <= 4 and svh.depth < _lib.MAX_DEPTH:
             call("nksr_gram_fill_grouped", svh.view(), self.feat_view(), cs, cnt, rowptr, place, col, val, rhs, diag, st)
+        elif place is not None and fill == "brick":
+            call("nksr_gram_fill_brick", svh.view(), self.feat_view(), cs, cnt, rowptr, place, col, val, rhs, diag,
+                 float(BRICK_MIN_LOCATIONS_PER_VOXEL), st)
         elif place is not None:
             call("nksr_gram_fill_placed", svh.view(), self.feat_view(), cs, cnt, rowptr, place, col, val, rhs, diag, st)
         else:
