@@ -290,6 +290,28 @@ NKSR_API int nksr_evaluate(const nksr_svh_t* svh, const nksr_feat_t* feat, const
                   const float* xyz, int64_t m, int want_grad, int approx_kernel_grad,
                   float* f, float* grad, void* stream);
 
+/* ---- a5b: backward of the kernel field (training through KernelField.solve / evaluate_f, models/nksr_net.py:91-112,
+ * models/loss.py:163-260).  Locations xyz are Morton SORTED, base[l*m + i] = their containing voxels
+ * (nksr_locate), range = nksr_row_ranges of every level concatenated in level order (read as int2 pairs: 8-byte
+ * aligned).  mode 0: value rows, 1: gradient
+ * rows (approx_kernel_grad: without the grad(phi) terms, as the forward).  Deterministic: no atomics, one fixed
+ * summation order.  ws: nksr_field_bwd_workspace_bytes(depth, m, C, mode, approx, feature_vjp) bytes (per-location
+ * phi / psi vectors), else NKSR_E_WORKSPACE. */
+NKSR_API size_t nksr_field_bwd_workspace_bytes(int depth, int64_t m, int channels, int mode, int approx_kernel_grad,
+                                               int feature_vjp);
+/* dalpha (all unknowns, overwritten) = sum_q coef_q E_q: coef (m) for value rows, (m,3) for gradient rows */
+NKSR_API int nksr_evaluate_adjoint(const nksr_svh_t* svh, const nksr_feat_t* feat, const float* xyz,
+                          const int32_t* base, const int32_t* range, int64_t m, int mode, int approx_kernel_grad,
+                          const float* coef, float* dalpha, void* ws, size_t ws_bytes, void* stream);
+/* dz (n_total x C, level blocks at svh->offset, ADDED to) += d/dz sum_q sum_s omega_{q,s} E_q[n_s], with
+ * omega_{q,(a,)s} = coef[q,0(,a)] a0[n_s] + coef[q,1(,a)] a1[n_s]; a1 may be NULL (coef then (m) or (m,3)) */
+NKSR_API int nksr_feature_vjp(const nksr_svh_t* svh, const nksr_feat_t* feat, const float* xyz, const int32_t* base,
+                     const int32_t* range, int64_t m, int mode, int approx_kernel_grad, const float* a0,
+                     const float* a1, const float* coef, float* dz, void* ws, size_t ws_bytes, void* stream);
+/* dz += w * d/dz (lam^T R alpha), R the regulariser of SPEC S5 without its weight */
+NKSR_API int nksr_regulariser_vjp(const nksr_svh_t* svh, const nksr_feat_t* feat, const float* lam,
+                         const float* alpha, float w, float* dz, void* stream);
+
 /* ---- a7: field.extract_dual_mesh (models/nksr_net.py:214,284; examples/recons_simple.py:27) ---- */
 /* flag[i]=1 if the dual cell with min corner voxel i exists (all 8 voxels active) */
 NKSR_API int nksr_mesh_cell_flags(const nksr_svh_t* svh, int32_t* flag, void* stream);

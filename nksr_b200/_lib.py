@@ -102,6 +102,10 @@ _SIGNATURES = {
     "nksr_gather_f32": ("i", "ppqpp"),
     "nksr_scatter_f32": ("i", "ppqpp"),
     "nksr_evaluate": ("i", "SFppqiippp"),
+    "nksr_field_bwd_workspace_bytes": ("z", "iqiiii"),
+    "nksr_evaluate_adjoint": ("i", "SFpppqii" + "pppzp"),
+    "nksr_feature_vjp": ("i", "SFpppqii" + "pppppzp"),
+    "nksr_regulariser_vjp": ("i", "SFppfpp"),
     "nksr_mesh_cell_flags": ("i", "Spp"),
     "nksr_mesh_stage0_cells": ("i", "Sppipp"),
     "nksr_mesh_leaf_flags": ("i", "Sipp"),

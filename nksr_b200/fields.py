@@ -84,8 +84,9 @@ class BaseField:
 
     def extract_dual_mesh(self, grid_upsample: int = 1, mise_iter: int = 0, max_points: int = -1, cell_filter=None):
         from .meshing import extract_dual_mesh
-        return extract_dual_mesh(self, grid_upsample=grid_upsample, mise_iter=mise_iter, max_points=max_points,
-                                 cell_filter=cell_filter)
+        with torch.no_grad():          # meshing records no graph, even of a field that is being trained
+            return extract_dual_mesh(self, grid_upsample=grid_upsample, mise_iter=mise_iter, max_points=max_points,
+                                     cell_filter=cell_filter)
 
 
 def _as_level_list(features, depth):
@@ -131,10 +132,16 @@ class KernelField(BaseField):
                 continue
             if f.shape[0] != n:
                 raise ValueError(f"features[{l}] has {f.shape[0]} rows but level {l} has {n} voxels")
-            f = f.detach().to(dev, torch.float32)
+            mod = None
             if self.interpolator is not None:
                 mod = self.interpolator[l] if not isinstance(self.interpolator, dict) else self.interpolator[str(l)]
-                with torch.no_grad():
+            # training: keep the interpolator's graph, so that the kernel solve / evaluation backpropagate into the
+            # basis features and the interpolator parameters (the same operations, so the same z)
+            graph = torch.is_grad_enabled() and (f.requires_grad or (
+                mod is not None and any(p.requires_grad for p in getattr(mod, "parameters", lambda: [])())))
+            f = (f if graph else f.detach()).to(dev, torch.float32)
+            if mod is not None:
+                with torch.set_grad_enabled(graph):
                     f = mod(f)
             f = f.contiguous()
             if f.data_ptr() % 16:                     # the kernels fetch four channels per 128-bit load
@@ -162,11 +169,9 @@ class KernelField(BaseField):
         return self._feat_view
 
     # ------------------------------------------------------------------ solve
-    def _sorted_rows(self, xyz: torch.Tensor, mode: int, extra: Optional[torch.Tensor] = None,
-                     interleaved: bool = False):
-        """Morton-sort locations, locate them on every level, build their kernel rows.
-        `interleaved` (depth <= 4, modes 0 / 1): rows as (m, rows, 32, 4 levels) -- the four levels of a slot are one
-        float4 -- instead of (m, depth, rows * 32)."""
+    def _sorted_locations(self, xyz: torch.Tensor, extra: Optional[torch.Tensor] = None):
+        """Morton-sort locations and locate them on every level: (perm, sorted xyz, sorted extra, base (depth, m),
+        ranges (n, 2): the first / last + 1 sorted location of every voxel, levels concatenated)."""
         svh, dev = self.svh, xyz.device
         st = stream_ptr(dev)
         m = xyz.shape[0]
@@ -185,6 +190,17 @@ class KernelField(BaseField):
         offs = svh.offsets
         for l in range(svh.depth):
             call("nksr_row_ranges", base[l], m, ranges[offs[l]:], svh.num_voxels(l), st)
+        return perm, xs, ex, base, ranges
+
+    def _sorted_rows(self, xyz: torch.Tensor, mode: int, extra: Optional[torch.Tensor] = None,
+                     interleaved: bool = False, loc=None):
+        """Morton-sort locations, locate them on every level, build their kernel rows.
+        `interleaved` (depth <= 4, modes 0 / 1): rows as (m, rows, 32, 4 levels) -- the four levels of a slot are one
+        float4 -- instead of (m, depth, rows * 32).  `loc`: the result of _sorted_locations, when the caller has it."""
+        svh, dev = self.svh, xyz.device
+        st = stream_ptr(dev)
+        m = xyz.shape[0]
+        _, xs, ex, base, ranges = loc if loc is not None else self._sorted_locations(xyz, extra)
         width = _lib.ROW_STRIDE * (3 if mode == 1 else 1)
         if interleaved:
             if svh.depth > 4 or mode == 2:
@@ -206,10 +222,29 @@ class KernelField(BaseField):
                  int(self.approx_kernel_grad), e, st)
         return xs, ex, base, ranges, e
 
+    def _wants_grad(self, *tensors):
+        return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (*self.z, *tensors))
+
     def solve(self, pos_xyz, normal_xyz=None, normal_value=None, pos_weight=1.0, normal_weight=1.0,
               reg_weight=1.0, fused_mode: bool = False):
-        """Assemble A = E^T W E + reg R (CSR) and solve A alpha = E^T W t with Jacobi-PCG."""
+        """Assemble A = E^T W E + reg R (CSR) and solve A alpha = E^T W t with Jacobi-PCG.
+        When grad is enabled and the features (or normal_value) require grad, alpha carries a graph: its backward runs
+        the adjoint solve and the feature-VJP kernels (_KernelSolve)."""
+        if self._wants_grad(normal_value if normal_xyz is not None else None):
+            nv = normal_value if normal_xyz is not None and normal_xyz.shape[0] > 0 else None
+            self.alpha = _KernelSolve.apply(self, (pos_xyz, normal_xyz, pos_weight, normal_weight, reg_weight), nv,
+                                            *self.z)
+            return self
         sysm = self.assemble(pos_xyz, normal_xyz, normal_value, pos_weight, normal_weight, reg_weight)
+        self.alpha = self._pcg(sysm, sysm.rhs)
+        if self.solver_config.get("keep_system"):
+            self.system = sysm
+        return self
+
+    def _pcg(self, sysm, rhs, adjoint: bool = False):
+        """Jacobi-PCG on the assembled system: the forward solve (A alpha = b) and the adjoint solve of the backward
+        (A lambda = dL/dalpha, the same symmetric matrix) share it.  A breakdown raises, max_iter warns; the forward
+        fills solve_info, the adjoint adds 'adjoint_iterations' / 'adjoint_relative_residual' to it."""
         dev, n = self.svh.device, sysm.n
         tm = getattr(self, "_timer", None) or _lib.StageTimer(dev, enabled=False)
         alpha = torch.empty(n, dtype=torch.float32, device=dev)
@@ -228,33 +263,34 @@ class KernelField(BaseField):
             offs = self.svh.offsets
             split_row = offs[2] if self.svh.depth > 2 else n
             split_nnz = int(sysm.rowptr[split_row].item()) if split_row < n else sysm.nnz
-            call("nksr_pcg_solve_stream", sysm.rowptr, sysm.col, sysm.val, sysm.diag, sysm.rhs, alpha, n, sysm.nnz,
+            call("nksr_pcg_solve_stream", sysm.rowptr, sysm.col, sysm.val, sysm.diag, rhs, alpha, n, sysm.nnz,
                  split_row, split_nnz, float(self.solver_config["tol"]), int(self.solver_config["max_iter"]),
                  int(self.solver_config["check_every"]), profile, ws, nb, info, stream_ptr(dev))
         else:
             nb = call("nksr_pcg_workspace_bytes", n)
             ws = torch.empty(nb, dtype=torch.uint8, device=dev)
-            call("nksr_pcg_solve", sysm.rowptr, sysm.col, sysm.val, sysm.diag, sysm.rhs, alpha, n,
+            call("nksr_pcg_solve", sysm.rowptr, sysm.col, sysm.val, sysm.diag, rhs, alpha, n,
                  float(self.solver_config["tol"]), int(self.solver_config["max_iter"]),
                  int(self.solver_config["check_every"]), profile, ws, nb, info, stream_ptr(dev))
-        tm.mark("pcg")
-        self.alpha = alpha
+        tm.mark("adjoint_pcg" if adjoint else "pcg")
         status = int(info[4])                       # 0 converged, 1 max_iter reached, 2 NaN / breakdown
-        self.solve_info = {"iterations": int(info[0]), "relative_residual": float(info[1]), "n": n, "nnz": sysm.nnz,
-                           "converged": status == 0}
+        if adjoint:
+            self.solve_info.update(adjoint_iterations=int(info[0]), adjoint_relative_residual=float(info[1]))
+        else:
+            self.solve_info = {"iterations": int(info[0]), "relative_residual": float(info[1]), "n": n,
+                               "nnz": sysm.nnz, "converged": status == 0}
+        what = "adjoint PCG" if adjoint else "PCG"
         if status == 2:
-            raise _lib.NksrError(f"PCG broke down (non-finite residual) after {int(info[0])} iterations: the system "
+            raise _lib.NksrError(f"{what} broke down (non-finite residual) after {int(info[0])} iterations: the system "
                                  "is not positive definite or the inputs are not finite")
         if status == 1 and int(self.solver_config["max_iter"]) > 0:
-            warnings.warn(f"nksr_b200 PCG stopped at max_iter={int(self.solver_config['max_iter'])} with relative "
+            warnings.warn(f"nksr_b200 {what} stopped at max_iter={int(self.solver_config['max_iter'])} with relative "
                           f"residual {float(info[1]):.3e} > tol={float(self.solver_config['tol']):.1e}", RuntimeWarning)
-        if profile:
+        if profile and not adjoint:
             self.solve_info.update(spmv_ms=float(info[2]), spmv_launches=int(info[3]))
         if self.solver_config.get("verbose"):
-            print(f"[nksr_b200] PCG: n={n} nnz={sysm.nnz} iters={int(info[0])} relres={float(info[1]):.3e}")
-        if self.solver_config.get("keep_system"):
-            self.system = sysm
-        return self
+            print(f"[nksr_b200] {what}: n={n} nnz={sysm.nnz} iters={int(info[0])} relres={float(info[1]):.3e}")
+        return alpha
 
     def _count_and_place(self, n, keep):
         """structure-only part of the assembly (row lengths, placement tables, row pointers): depends on the hierarchy
@@ -298,8 +334,10 @@ class KernelField(BaseField):
         return cnt, cnt_down, place, rowptr
 
     def assemble(self, pos_xyz, normal_xyz=None, normal_value=None, pos_weight=1.0, normal_weight=1.0,
-                 reg_weight=1.0):
-        """Kernel rows + Gram assembly: returns the CSR system (rowptr, col, val, rhs, diag, n, nnz)."""
+                 reg_weight=1.0, keep_constraints: bool = False):
+        """Kernel rows + Gram assembly: returns the CSR system (rowptr, col, val, rhs, diag, n, nnz).
+        keep_constraints: also `.cons`, the sorted constraint locations, their containing voxels and ranges, the
+        sorted normal targets and the weights -- what the backward needs (it rebuilds no kernel row from E)."""
         svh = self.svh
         dev = svh.device
         _lib.require_cuda(pos_xyz, "pos_xyz")
@@ -334,7 +372,11 @@ class KernelField(BaseField):
         ilv = (layout == "interleaved" and svh.depth <= 4 and not (self.approx_kernel_grad and compact)
                and (self.solver_config.get("fill") or os.environ.get("NKSR_FILL") or DEFAULT_FILL) in ("rows", "brick")
                and (self.solver_config.get("rows") or os.environ.get("NKSR_ROWS") or "location") == "location")
-        _, _, _, range_pos, e_pos = self._sorted_rows(pos_xyz, 0, interleaved=ilv)
+        loc_pos = self._sorted_locations(pos_xyz)
+        _, _, _, range_pos, e_pos = self._sorted_rows(pos_xyz, 0, interleaved=ilv, loc=loc_pos)
+        cons = SimpleNamespace(pos=(loc_pos[1], loc_pos[3], loc_pos[4]),
+                               nrm=None, perm_nrm=None, w_pos=float(pos_weight), w_nrm=float(normal_weight),
+                               w_reg=float(reg_weight)) if keep_constraints else None
         keep += [range_pos, e_pos]
         cs.e_pos, cs.range_pos, cs.n_pos, cs.w_pos = e_pos.data_ptr(), range_pos.data_ptr(), pos_xyz.shape[0], float(pos_weight)
         if normal_xyz is not None and normal_xyz.shape[0] > 0:
@@ -344,7 +386,11 @@ class KernelField(BaseField):
             # compact gradient rows (one line instead of three per location and level) save 2/3 of
             # the row memory but cost ALU in the assembly, so they are opt-in for clouds that would not fit otherwise
             nrm_mode = 2 if (self.approx_kernel_grad and compact) else 1
-            _, t_nrm, _, range_nrm, e_nrm = self._sorted_rows(normal_xyz, nrm_mode, normal_value, interleaved=ilv)
+            loc_nrm = self._sorted_locations(normal_xyz, normal_value)
+            _, t_nrm, _, range_nrm, e_nrm = self._sorted_rows(normal_xyz, nrm_mode, normal_value, interleaved=ilv,
+                                                              loc=loc_nrm)
+            if cons is not None:
+                cons.nrm, cons.t_nrm, cons.perm_nrm = (loc_nrm[1], loc_nrm[3], loc_nrm[4]), t_nrm, loc_nrm[0]
             cs.nrm_compact = 2 if ilv else int(nrm_mode == 2)          # the C struct's row-layout code
             keep += [t_nrm, range_nrm, e_nrm]
             cs.e_nrm, cs.range_nrm, cs.t_nrm = e_nrm.data_ptr(), range_nrm.data_ptr(), t_nrm.data_ptr()
@@ -431,7 +477,7 @@ class KernelField(BaseField):
         del keep
         tm.mark("gram_sort")
         return SimpleNamespace(rowptr=rowptr, col=col, val=val, rhs=rhs, diag=diag, cnt=cnt, cnt_down=cnt_down,
-                               n=n, nnz=nnz)
+                               n=n, nnz=nnz, cons=cons)
 
     # the reference exposes both spellings; both run the same fused assembly here
     def solve_non_fused(self, pos_xyz, normal_xyz, normal_value, pos_weight, normal_weight, reg_weight):
@@ -439,16 +485,64 @@ class KernelField(BaseField):
 
     # ------------------------------------------------------------------ evaluation
     def evaluate_f(self, xyz: torch.Tensor, grad: bool = False) -> EvaluationResult:
+        """f (and grad f) at xyz.  When grad is enabled and alpha or the features require grad, the result carries a
+        graph into alpha and the features (_KernelEvaluate); query positions get no gradient."""
         if self.alpha is None:
             raise _lib.NksrError("KernelField.evaluate_f called before solve()")
         _lib.require_cuda(xyz, "xyz")
         xyz = xyz.detach().to(self.svh.device, torch.float32).contiguous()
+        if self._wants_grad(self.alpha):
+            out = _KernelEvaluate.apply(self, xyz, bool(grad), self.alpha, *self.z)
+            return EvaluationResult(value=out[0], gradient=out[1] if grad else None)
+        f, g = self._evaluate(self.alpha, xyz, grad)
+        return EvaluationResult(value=f, gradient=g)
+
+    def _evaluate(self, alpha, xyz, grad):
         m = xyz.shape[0]
         f = torch.empty(m, dtype=torch.float32, device=xyz.device)
         g = torch.empty((m, 3), dtype=torch.float32, device=xyz.device) if grad else None
-        call("nksr_evaluate", self.svh.view(), self.feat_view(), self.alpha, xyz, m, int(grad),
+        call("nksr_evaluate", self.svh.view(), self.feat_view(), alpha, xyz, m, int(grad),
              int(self.approx_kernel_grad), f, g, stream_ptr(xyz.device))
-        return EvaluationResult(value=f, gradient=g)
+        return f, g
+
+    # ------------------------------------------------------------------ backward (DESIGN 4.6)
+    def _query_locations(self, xyz):
+        """sorted locations of the queries the forward can evaluate (finite, inside the key range); the others
+        evaluate to 0 and get no gradient.  Returns (index into xyz, sorted xyz, base, ranges)."""
+        half = self.svh.voxel_size * 0.5
+        ok = torch.isfinite(xyz).all(dim=1) & ((xyz / half).abs() < float(2 ** 20 - 64)).all(dim=1)
+        keep = torch.nonzero(ok).reshape(-1)
+        q = xyz[keep].contiguous()
+        perm, xs, _, base, ranges = self._sorted_locations(q)
+        return keep[perm], xs, base, ranges
+
+    def _feature_vjp(self, loc, mode, coef, a0, a1, dz):
+        """dz (n, C) += d/dz sum_q sum_s omega_{q,s} E_q[n_s] at the sorted locations `loc` = (xs, base, ranges)"""
+        xs, base, ranges = loc
+        m = xs.shape[0]
+        if m == 0:
+            return
+        nb = call("nksr_field_bwd_workspace_bytes", self.svh.depth, m, self.channels, mode,
+                  int(self.approx_kernel_grad), 1)
+        ws = _lib._ws(nb, xs.device)
+        call("nksr_feature_vjp", self.svh.view(), self.feat_view(), xs, base, ranges, m, mode,
+             int(self.approx_kernel_grad), a0, a1, coef.contiguous(), dz, ws, nb, stream_ptr(xs.device))
+
+    def _evaluate_adjoint(self, loc, mode, coef):
+        """dalpha = sum_q coef_q E_q at the sorted locations `loc`"""
+        xs, base, ranges = loc
+        m = xs.shape[0]
+        dalpha = torch.empty(self.svh.num_unknowns, dtype=torch.float32, device=self.svh.device)
+        nb = call("nksr_field_bwd_workspace_bytes", self.svh.depth, m, self.channels, mode,
+                  int(self.approx_kernel_grad), 0)
+        ws = _lib._ws(nb, dalpha.device)
+        call("nksr_evaluate_adjoint", self.svh.view(), self.feat_view(), xs, base, ranges, m, mode,
+             int(self.approx_kernel_grad), coef.contiguous(), dalpha, ws, nb, stream_ptr(dalpha.device))
+        return dalpha
+
+    def _level_grads(self, dz):
+        offs = self.svh.offsets
+        return tuple(dz[offs[l]:offs[l] + self.svh.num_voxels(l)] for l in range(self.svh.depth))
 
     def evaluate_f_bar(self, xyz: torch.Tensor) -> torch.Tensor:
         """Occupancy-style value (> 0 inside, models/loss.py:99); masked-out regions read as outside."""
@@ -468,6 +562,101 @@ class KernelField(BaseField):
             self.alpha = self.alpha.to(device)
         self._feat_view = None
         return self
+
+
+class _KernelSolve(torch.autograd.Function):
+    """alpha = A(z)^-1 b(z, t).  Forward: the assembly and PCG of KernelField.solve (the same alpha, bit for bit).
+    Backward, with lambda = A^-1 dL/dalpha (one more PCG on the same symmetric matrix):
+      dL/dz   = sum_j w_j [(t_j - E_j alpha) d(E_j lambda) - (E_j lambda) d(E_j alpha)] - reg d(lambda^T R alpha)
+      dL/dt_j = w_j E_j lambda                                                     (the normal rows' targets)
+    The first line is a row functional with omega = c^lambda lambda + c^alpha alpha per row (nksr_feature_vjp); the
+    E_j alpha, E_j lambda are field evaluations at the constraint locations.  E itself is not kept."""
+
+    @staticmethod
+    def forward(ctx, field, args, normal_value, *z):
+        pos_xyz, normal_xyz, pos_weight, normal_weight, reg_weight = args
+        sysm = field.assemble(pos_xyz, normal_xyz, normal_value, pos_weight, normal_weight, reg_weight,
+                              keep_constraints=True)
+        alpha = field._pcg(sysm, sysm.rhs)
+        if field.solver_config.get("keep_system"):
+            field.system = sysm
+        ctx.field, ctx.sysm = field, sysm
+        ctx.save_for_backward(alpha)
+        return alpha
+
+    @staticmethod
+    def backward(ctx, g_alpha):
+        field, sysm = ctx.field, ctx.sysm
+        (alpha,) = ctx.saved_tensors
+        cons = sysm.cons
+        tm = getattr(field, "_timer", None) or _lib.StageTimer(alpha.device, enabled=False)
+        tm.mark("backward_start")
+        g_alpha = g_alpha.detach().to(torch.float32).contiguous()
+        if bool((g_alpha != 0).any()):
+            lam = field._pcg(sysm, g_alpha, adjoint=True)
+        else:
+            lam = torch.zeros_like(alpha)
+            field.solve_info.update(adjoint_iterations=0, adjoint_relative_residual=0.0)
+        n, C_ = sysm.n, field.channels
+        dz = torch.zeros((n, C_), dtype=torch.float32, device=alpha.device)
+        xs, base, ranges = cons.pos
+        f_a, _ = field._evaluate(alpha, xs, False)
+        f_l, _ = field._evaluate(lam, xs, False)
+        coef = torch.stack([-cons.w_pos * f_a, -cons.w_pos * f_l], dim=1)         # omega = c^lam lam + c^alpha alpha
+        field._feature_vjp(cons.pos, 0, coef, lam, alpha, dz)
+        d_nv = None
+        if cons.nrm is not None:
+            xs_n = cons.nrm[0]
+            _, g_a = field._evaluate(alpha, xs_n, True)
+            _, g_l = field._evaluate(lam, xs_n, True)
+            coef = torch.stack([cons.w_nrm * (cons.t_nrm - g_a), -cons.w_nrm * g_l], dim=1)     # (k, 2, 3)
+            field._feature_vjp(cons.nrm, 1, coef, lam, alpha, dz)
+            if ctx.needs_input_grad[2]:                                             # back to the caller's order
+                d_nv = torch.empty_like(g_l)
+                d_nv[cons.perm_nrm] = cons.w_nrm * g_l
+        if cons.w_reg != 0.0:
+            call("nksr_regulariser_vjp", field.svh.view(), field.feat_view(), lam, alpha, -cons.w_reg, dz,
+                 stream_ptr(alpha.device))
+        tm.mark("feature_vjp")
+        ctx.field = ctx.sysm = None          # (field.alpha -> this node -> field: do not keep the system alive)
+        return (None, None, d_nv) + field._level_grads(dz)
+
+
+class _KernelEvaluate(torch.autograd.Function):
+    """(f, grad f) = E(z, xyz) alpha.  Forward: nksr_evaluate (the same values as without grad).  Backward:
+    dL/dalpha = sum_q g_q E_q (nksr_evaluate_adjoint); dL/dz = the row functional with omega = g_q alpha
+    (nksr_feature_vjp), for the value and the gradient rows."""
+
+    @staticmethod
+    def forward(ctx, field, xyz, grad, alpha, *z):
+        f, g = field._evaluate(alpha, xyz, grad)
+        ctx.field, ctx.xyz, ctx.grad = field, xyz, grad
+        ctx.save_for_backward(alpha)
+        return (f, g) if grad else (f,)
+
+    @staticmethod
+    def backward(ctx, g_f, g_g=None):
+        field = ctx.field
+        (alpha,) = ctx.saved_tensors
+        tm = getattr(field, "_timer", None) or _lib.StageTimer(alpha.device, enabled=False)
+        tm.mark("evaluate_backward_start")
+        n = field.svh.num_unknowns
+        idx, xs, base, ranges = field._query_locations(ctx.xyz)
+        loc = (xs, base, ranges)
+        d_alpha = torch.zeros(n, dtype=torch.float32, device=alpha.device)
+        dz = torch.zeros((n, field.channels), dtype=torch.float32, device=alpha.device)
+        want_z = any(ctx.needs_input_grad[4:])
+        for mode, g in ((0, g_f), (1, g_g if ctx.grad else None)):
+            if g is None:
+                continue
+            coef = g.detach().to(torch.float32)[idx].contiguous()
+            if ctx.needs_input_grad[3]:
+                d_alpha += field._evaluate_adjoint(loc, mode, coef)
+            if want_z:
+                field._feature_vjp(loc, mode, coef, alpha, None, dz)
+        tm.mark("evaluate_vjp")
+        ctx.field = ctx.xyz = None
+        return (None, None, None, d_alpha) + field._level_grads(dz)
 
 
 class LayerField(BaseField):

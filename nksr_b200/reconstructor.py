@@ -328,6 +328,11 @@ class Reconstructor:
             feat = view / (torch.linalg.norm(view, dim=-1, keepdim=True) + 1e-6)     # models/nksr_net.py:48-52
         else:
             raise ValueError("either normal or sensor (with a normal-estimating preprocess_fn) is required")
+        with torch.no_grad():        # reconstruction is inference: no graph, no system kept, even for a trainable network
+            return self._reconstruct_field(xyz, feat, voxel_size, approx_kernel_grad, solver_tol, fused_mode,
+                                           solver_max_iter)
+
+    def _reconstruct_field(self, xyz, feat, voxel_size, approx_kernel_grad, solver_tol, fused_mode, solver_max_iter):
         tm = self._timer
         svh = SparseFeatureHierarchy(voxel_size, self.tree_depth, self.device).build_point_splatting(xyz)
         tm.mark("svh_build")

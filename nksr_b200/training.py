@@ -1,7 +1,8 @@
-"""Training losses of the U-Net backbone that need only the network's backward (not a backward through the kernel
-solve): the structure loss and the UDF loss of the reference (models/loss.py:143-160 and :106-140), with the samplers
-and ground-truth transform of configs/default/train.yaml (supervision.structure_weight, supervision.udf,
-supervision.spatial.gt_band / gt_soft).
+"""Training losses of the U-Net backbone: the structure loss and the UDF loss of the reference (models/loss.py:143-160
+and :106-140), with the samplers and ground-truth transform of configs/default/train.yaml
+(supervision.structure_weight, supervision.udf, supervision.spatial.gt_band / gt_soft), and -- opt-in,
+`train_step(..., kernel=True)` -- the kernel-field losses, which backpropagate through the kernel solve
+(supervision.gt_surface and supervision.spatial, models/loss.py:163-260; fields._KernelSolve).
 
     feat, dec_svh, _ = net.unet(net.encoder(xyz, normal, svh, 0), svh)
     l_struct, per_level = structure_loss(feat.structure_features, dec_svh, gt_svh)
@@ -15,7 +16,7 @@ from __future__ import annotations
 import torch
 import torch.nn.functional as F
 
-from .fields import NeuralField
+from .fields import KernelField, NeuralField
 from .sdfgen import sdf_from_points
 from .svh import SparseFeatureHierarchy
 
@@ -25,6 +26,15 @@ UDF_WEIGHT = 150.0
 UDF_SAMPLERS = (dict(type="uniform", n_samples=80000, expand=1, expand_top=5),
                 dict(type="band", n_samples=20000, eps=0.5))
 GT_BAND = 1.0
+# supervision.gt_surface (value / normal weights, subsample) and supervision.spatial (weight, samplers); solver weights
+GT_SURFACE_VALUE_WEIGHT = 200.0
+GT_SURFACE_NORMAL_WEIGHT = 100.0
+GT_SURFACE_SUBSAMPLE = 50000
+SPATIAL_WEIGHT = 300.0
+SPATIAL_SAMPLERS = (dict(type="uniform", n_samples=50000, expand=1, expand_top=3),
+                    dict(type="band", n_samples=50000, eps=0.5))
+POS_WEIGHT = 1.0e4
+NORMAL_WEIGHT = 1.0e4
 
 
 def structure_loss(structure_features, dec_svh: SparseFeatureHierarchy, gt_svh: SparseFeatureHierarchy):
@@ -122,14 +132,69 @@ class TrainingScene:
         self.adaptive_depth = adaptive_depth
 
 
-def losses(net, scene: TrainingScene, generator=None):
-    """forward of a trainable NKSRNetwork on the scene and its weighted losses: (total, structure, udf)"""
+def kernel_field(net, feat, dec_svh: SparseFeatureHierarchy, scene: TrainingScene, timer=None):
+    """the KernelField of models/nksr_net.py:91-112: basis features through the interpolators, position constraints at
+    the input points, normal constraints (value -normal_features) at the voxel centres of the `adaptive_depth` finest
+    levels, solved with the solver weights of train.yaml.  Differentiable when grad is enabled (fields._KernelSolve)."""
+    field = KernelField(dec_svh, net.interpolators, feat.basis_features)
+    if timer is not None:
+        field._timer = timer
+        timer.mark("solve_start")
+    ad = min(scene.adaptive_depth, dec_svh.depth)
+    normal_xyz = torch.cat([dec_svh.get_voxel_centers(d) for d in range(ad)])
+    normal_value = torch.cat([feat.normal_features[d] for d in range(ad)])
+    normal_weight = NORMAL_WEIGHT / normal_xyz.shape[0] * (scene.voxel_size ** 2)
+    field.solve(scene.xyz, normal_xyz, -normal_value, POS_WEIGHT / scene.xyz.shape[0], normal_weight, 1.0)
+    return field
+
+
+def gt_surface_loss(field, ref_xyz, ref_normal, subsample=GT_SURFACE_SUBSAMPLE, generator=None):
+    """(value, normal) losses at a subsample of the reference points (models/loss.py:163-198): mean |f| and
+    1 - mean <-grad f / |grad f|, n>"""
+    if 0 < subsample < ref_xyz.shape[0]:
+        idx = (torch.rand((subsample,), device=ref_xyz.device, generator=generator) * ref_xyz.shape[0]).long()
+    else:
+        idx = torch.arange(ref_xyz.shape[0], device=ref_xyz.device)
+    ev = field.evaluate_f(ref_xyz[idx], grad=True)
+    g = -ev.gradient / (torch.linalg.norm(ev.gradient, dim=-1, keepdim=True) + 1.0e-6)
+    return ev.value.abs().mean(), 1.0 - torch.sum(g * ref_normal[idx], dim=-1).mean()
+
+
+def spatial_loss(field, ref_xyz, ref_normal, voxel_size, samplers=SPATIAL_SAMPLERS, gt_band=GT_BAND, generator=None):
+    """near-surface L1 of the transformed field against the transformed point-cloud SDF, / voxel_size, over the uniform +
+    band samples (models/loss.py:201-260).  Without GT geometry every sample counts as near-surface."""
+    q = udf_samples(field.svh, ref_xyz, ref_normal, voxel_size, samplers, generator)
+    gt = transform_field(-sdf_from_points(q, ref_xyz, ref_normal, 8, 0.02, False)[0], voxel_size, gt_band)
+    pd = transform_field(field.evaluate_f(q).value, voxel_size, gt_band)
+    return torch.sum(torch.abs((pd - gt) / voxel_size)) / q.shape[0]
+
+
+def kernel_losses(net, scene: TrainingScene, generator=None, feat=None, dec_svh=None, timer=None):
+    """the kernel-field losses of a trainable NKSRNetwork on the scene: dict(total, gt_value, gt_normal, spatial,
+    field).  `feat`, `dec_svh`: an existing forward of the network (else one is run)."""
+    if feat is None:
+        enc = net.encoder(scene.xyz, scene.normal, scene.enc_svh, 0)
+        feat, dec_svh, _ = net.unet(enc, scene.enc_svh, adaptive_depth=scene.adaptive_depth)
+    field = kernel_field(net, feat, dec_svh, scene, timer)
+    l_val, l_nrm = gt_surface_loss(field, scene.xyz, scene.normal, generator=generator)
+    l_sp = spatial_loss(field, scene.xyz, scene.normal, scene.voxel_size, generator=generator)
+    total = GT_SURFACE_VALUE_WEIGHT * l_val + GT_SURFACE_NORMAL_WEIGHT * l_nrm + SPATIAL_WEIGHT * l_sp
+    return dict(total=total, gt_value=l_val, gt_normal=l_nrm, spatial=l_sp, field=field)
+
+
+def losses(net, scene: TrainingScene, generator=None, kernel=False, timer=None):
+    """forward of a trainable NKSRNetwork on the scene and its weighted losses: (total, structure, udf), and with
+    `kernel` the kernel_losses dict as a fourth element (its total is included in the first)"""
     enc = net.encoder(scene.xyz, scene.normal, scene.enc_svh, 0)
     feat, dec_svh, _ = net.unet(enc, scene.enc_svh, adaptive_depth=scene.adaptive_depth)
     l_struct, _ = structure_loss(feat.structure_features, dec_svh, scene.gt_svh)
     l_udf = udf_loss(net.udf_decoder, feat.udf_features, dec_svh, scene.xyz, scene.normal, scene.voxel_size,
                      generator=generator)
-    return STRUCTURE_WEIGHT * l_struct + UDF_WEIGHT * l_udf, l_struct, l_udf
+    total = STRUCTURE_WEIGHT * l_struct + UDF_WEIGHT * l_udf
+    if not kernel:
+        return total, l_struct, l_udf
+    k = kernel_losses(net, scene, generator, feat, dec_svh, timer)
+    return total + k["total"], l_struct, l_udf, k
 
 
 GRAD_CLIP = 0.5         # configs/default/train.yaml: grad_clip
@@ -140,11 +205,14 @@ def make_optimizer(net):
     return torch.optim.Adam([p for p in net.parameters() if p.requires_grad], lr=LEARNING_RATE)
 
 
-def train_step(net, opt, scene: TrainingScene, generator=None, marks=None):
-    """one Adam step (gradient norm clipped to GRAD_CLIP); returns the (structure, udf) losses as tensors.  `marks`,
-    if given, is called with 'forward' / 'backward' / 'step' after each phase has been enqueued."""
+def train_step(net, opt, scene: TrainingScene, generator=None, marks=None, kernel=False, timer=None):
+    """one Adam step (gradient norm clipped to GRAD_CLIP); returns the (structure, udf) losses as tensors, and with
+    `kernel` (the kernel-field losses added, trained through the kernel solve) a third element: the dict of the
+    detached kernel losses.  `marks`, if given, is called with 'forward' / 'backward' / 'step' after each phase has
+    been enqueued; `timer` (a StageTimer) receives the kernel solve's stage marks."""
     opt.zero_grad(set_to_none=True)
-    total, l_struct, l_udf = losses(net, scene, generator)
+    out = losses(net, scene, generator, kernel, timer)
+    total, l_struct, l_udf = out[:3]
     if marks:
         marks("forward")
     total.backward()
@@ -154,4 +222,7 @@ def train_step(net, opt, scene: TrainingScene, generator=None, marks=None):
     opt.step()
     if marks:
         marks("step")
+    if kernel:
+        k = {key: v.detach() for key, v in out[3].items() if key != "field"}
+        return l_struct.detach(), l_udf.detach(), k
     return l_struct.detach(), l_udf.detach()

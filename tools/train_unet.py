@@ -3,12 +3,16 @@ the structure and UDF losses (nksr_b200/training.py), Adam lr 1e-4, gradient nor
 
     python tools/train_unet.py --scene sphere --points 200000 --steps 30 --precision fp32 --out ckpt.pt
     python tools/train_unet.py --scene cfg4 --points 1000000 --depth 4 --precision tc --steps 10
+    python tools/train_unet.py --scene cfg4 --points 1000000 --depth 4 --kernel-losses --steps 10
 
 Scenes: 'sphere' (tests/clouds.py, exact normals) or 'cfg4' (a crop of bench.py's outdoor scene at its own density,
 normals from the kNN preprocess).  Every step prints one JSON line: the losses and the CUDA-event times of the forward,
 the backward (with the sparse convolution's input-gradient and weight-gradient kernels separately) and the optimizer
 step.  The last line is a summary over the steps after the first two: median times, the weight-gradient kernel's
 achieved TFLOP/s (2 nnz_taps c_in c_out per call) and GB/s per (c_in, c_out) shape, and the GPU's name and power limit.
+--kernel-losses adds the kernel-field losses (GT-surface value / normal, spatial TSDF), trained through the kernel solve,
+and reports them per step with the CUDA-event times of the forward solve (assembly + PCG), the adjoint PCG and the VJP
+kernels (with the field evaluations they need).
 --out saves {'state_dict': ...}, which load_checkpoint_from_url(<path>) + load_state_dict take."""
 import argparse
 import json
@@ -94,6 +98,7 @@ def main(argv=None):
     ap.add_argument("--steps", type=int, default=30)
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--out", default=None, help="checkpoint path ({'state_dict': ...})")
+    ap.add_argument("--kernel-losses", action="store_true", help="add the kernel-field losses (train through the solve)")
     args = ap.parse_args(argv)
     if args.steps < 1:
         ap.error("--steps must be >= 1")
@@ -101,6 +106,7 @@ def main(argv=None):
     if not torch.cuda.is_available():
         raise SystemExit("train_unet.py needs a CUDA device")
     import nksr_b200.unet as U
+    from nksr_b200._lib import StageTimer
     from bench import gpu_info
     from nksr_b200 import training as T
     from nksr_b200.network import NKSRNetwork
@@ -127,11 +133,21 @@ def main(argv=None):
             ev[name].record()
             timer.phase = {"forward": "backward", "backward": "step"}.get(name, "forward")
         timer.phase = "forward"
-        l_struct, l_udf = T.train_step(net, opt, scene, gen, marks)
+        stages = StageTimer(dev, enabled=True) if args.kernel_losses else None
+        out = T.train_step(net, opt, scene, gen, marks, kernel=args.kernel_losses, timer=stages)
+        l_struct, l_udf = out[:2]
         timer.phase = "forward"
         torch.cuda.synchronize()
         k = timer.summary()
-        row = dict(step=step, structure=round(float(l_struct), 6), udf=round(float(l_udf), 6),
+        kern = {}
+        if args.kernel_losses:
+            st = stages.report()
+            kern = {name: round(float(v), 6) for name, v in out[2].items()}
+            kern.update(kernel_solve_ms=round(sum(st.get(s, 0.0) for s in ("kernel_rows", "gram_count", "gram_blocks",
+                                                                           "gram_fill", "gram_sort", "pcg")), 3),
+                        adjoint_pcg_ms=round(st.get("adjoint_pcg", 0.0), 3),
+                        vjp_ms=round(st.get("feature_vjp", 0.0) + st.get("evaluate_vjp", 0.0), 3))
+        row = dict(step=step, structure=round(float(l_struct), 6), udf=round(float(l_udf), 6), **kern,
                    forward_ms=round(ev["start"].elapsed_time(ev["forward"]), 3),
                    backward_ms=round(ev["forward"].elapsed_time(ev["backward"]), 3),
                    dgrad_ms=round(k["dgrad"], 3), wgrad_ms=round(k["wgrad"], 3),
@@ -140,7 +156,8 @@ def main(argv=None):
         print(json.dumps(row), flush=True)
     timed = rows[2:] if len(rows) > 2 else rows
     med = {key: round(statistics.median(r[key] for r in timed), 3)
-           for key in ("forward_ms", "backward_ms", "dgrad_ms", "wgrad_ms", "step_ms")}
+           for key in ("forward_ms", "backward_ms", "dgrad_ms", "wgrad_ms", "step_ms", "kernel_solve_ms",
+                       "adjoint_pcg_ms", "vjp_ms") if key in timed[0]}
     med["backward_over_forward"] = round(med["backward_ms"] / med["forward_ms"], 3)
     print(json.dumps(dict(summary=med, wgrad_last_step=timer.wgrad_rates(), **info)), flush=True)
     if args.out:
