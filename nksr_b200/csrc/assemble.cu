@@ -325,11 +325,7 @@ k_gram_fill(nksr_svh_t svh, nksr_feat_t feat, nksr_constraints_t cs, int64_t row
     if (rp) { my_pb = __ldg(rp + 2 * (int64_t)my_u); my_pe = __ldg(rp + 2 * (int64_t)my_u + 1); }
     if (rn) { my_nb = __ldg(rn + 2 * (int64_t)my_u); my_ne = __ldg(rn + 2 * (int64_t)my_u + 1); }
   }
-  // quadratic B-spline as polynomials in tau for this lane's offset d (SPEC S4):
-  // b = c0 + tau (c1 + c2 tau), db = c1 + 2 c2 tau
-  const float cx0 = ldx == 0 ? 0.75f : 0.125f, cx1 = 0.5f * (float)ldx, cx2 = ldx == 0 ? -1.f : 0.5f;
-  const float cy0 = ldy == 0 ? 0.75f : 0.125f, cy1 = 0.5f * (float)ldy, cy2 = ldy == 0 ? -1.f : 0.5f;
-  const float cz0 = ldz == 0 ? 0.75f : 0.125f, cz1 = 0.5f * (float)ldz, cz2 = ldz == 0 ? -1.f : 0.5f;
+  const CompactSpline spline(ldx, ldy, ldz);
   const float inv_wl = 1.f / (svh.voxel_size * (float)(1 << l));
   // rows are stored location-major ([q][L][rows][32]): level stride is a compile-time constant
   constexpr int pos_level = NKSR_ROW_STRIDE;
@@ -412,13 +408,8 @@ k_gram_fill(nksr_svh_t svh, nksr_feat_t feat, nksr_constraints_t cs, int64_t row
           if (k <= nup) {
             const float line = __ldg(pk);
             pk += nrm_level;
-            const float tx = __shfl_sync(0xffffffffu, line, 27), ty = __shfl_sync(0xffffffffu, line, 28),
-                        tz = __shfl_sync(0xffffffffu, line, 29);
-            const float bx = fmaf(fmaf(cx2, tx, cx1), tx, cx0), dbx = fmaf(2.f * cx2, tx, cx1);
-            const float by = fmaf(fmaf(cy2, ty, cy1), ty, cy0), dby = fmaf(2.f * cy2, ty, cy1);
-            const float bz = fmaf(fmaf(cz2, tz, cz1), tz, cz0), dbz = fmaf(2.f * cz2, tz, cz1);
-            const float sc = (lane < 27 ? line : 0.f) * iw;
-            const float e0 = dbx * by * bz * sc, e1 = bx * dby * bz * sc, e2 = bx * by * dbz * sc;
+            float e0, e1, e2;
+            spline.grad_rows(line, iw, lane, e0, e1, e2);
             if (k == 0) {
               a0 = cs.w_nrm * __shfl_sync(0xffffffffu, e0, si);
               a1 = cs.w_nrm * __shfl_sync(0xffffffffu, e1, si);

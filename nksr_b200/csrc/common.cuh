@@ -54,6 +54,29 @@ __host__ __device__ __forceinline__ int level_offset(int level) { return 1 << (1
 #define NKSR_HALF_OFFSET (1 << 20)
 #define NKSR_KEY_LIMIT (1 << 21)
 
+// The one device definition of the half-voxel quantisation (SPEC S1): h = floor(p / half_w) + 2^20 per axis, with
+// IEEE division.  p is relative to the keys' origin (callers with an origin subtract it first).  Returns false when an
+// axis is outside (-(2^20 - 16), 2^20 - 16) or NaN; that axis then gets h = 2^20.  The containing voxel on level l is
+// h >> (l+1).
+__device__ __forceinline__ bool half_voxel(float px, float py, float pz, float half_w, int3& h) {
+  const float p[3] = {px, py, pz};
+  int u[3];
+  bool bad = false;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    float q = floorf(__fdiv_rn(p[a], half_w));
+    if (!(q > -(float)(NKSR_HALF_OFFSET - 16) && q < (float)(NKSR_HALF_OFFSET - 16))) { bad = true; q = 0.f; }
+    u[a] = (int)q + NKSR_HALF_OFFSET;
+  }
+  h = make_int3(u[0], u[1], u[2]);
+  return !bad;
+}
+
+// slot in child8[s] (the table of level s) of the level-(s-1) voxel that contains half-voxel coordinates h
+__device__ __forceinline__ int child_octant(const int3& h, int s) {
+  return (((h.x >> s) & 1) << 2) | (((h.y >> s) & 1) << 1) | ((h.z >> s) & 1);
+}
+
 // lower_bound over sorted keys; returns index or -1 when absent
 __device__ __forceinline__ int find_key(const int64_t* __restrict__ keys, int64_t n, int64_t k) {
   int64_t lo = 0, hi = n;

@@ -27,12 +27,10 @@ k_build_rows(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ xyz, co
   constexpr bool GRAD = MODE == 1;
   constexpr int ROWS = GRAD ? 3 : 1;
   const float px = __ldg(xyz + 3 * i), py = __ldg(xyz + 3 * i + 1), pz = __ldg(xyz + 3 * i + 2);
-  // half-voxel coordinates of the point (SPEC S1, same expression as nksr_locate): the containing voxel on
-  // level l is (h + 2^20) >> (l+1), so no key has to be loaded and decoded per level
-  const float half_w = svh.voxel_size * 0.5f;
-  const int hx = (int)floorf(__fdiv_rn(px, half_w)) + NKSR_HALF_OFFSET;
-  const int hy = (int)floorf(__fdiv_rn(py, half_w)) + NKSR_HALF_OFFSET;
-  const int hz = (int)floorf(__fdiv_rn(pz, half_w)) + NKSR_HALF_OFFSET;
+  // half-voxel coordinates of the point: the containing voxel on level l is h >> (l+1), so no key has to be loaded
+  // and decoded per level.  A point outside the range has base -1 on every level (nksr_locate), so h is never read.
+  int3 h;
+  half_voxel(px, py, pz, svh.voxel_size * 0.5f, h);
   const double inv0 = 1.0 / (double)svh.voxel_size;
   // location-major layout [m][L][rows][32]: all lines of one location are contiguous, so the
   // assembly kernel reaches them with compile-time offsets from one base pointer
@@ -55,7 +53,7 @@ k_build_rows(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ xyz, co
       } else {
         const float wl = svh.voxel_size * (float)(1 << l);
         LaneKernel r = eval_level_lane<GRAD>(svh.nbr27[l], feat.z[l], feat.channels, l, wl, inv0, px, py, pz, b,
-                                             hx >> (l + 1), hy >> (l + 1), hz >> (l + 1), fullgrad, lane);
+                                             h.x >> (l + 1), h.y >> (l + 1), h.z >> (l + 1), fullgrad, lane);
         if (ILV) {
 #pragma unroll
           for (int a = 0; a < ROWS; ++a) kv[l][a] = GRAD ? r.dk[a] : r.k;
@@ -84,7 +82,7 @@ k_build_rows(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ xyz, co
 // above re-gathers 27 feature rows per location and level -- 27 L1 wavefronts per channel load, the measured limit of
 // that kernel; here the stencil and the features (C <= 16, as float4
 // registers) are fetched ONCE per voxel and the loop over the voxel's locations is ALU + shuffles + the row stores.
-// Same arithmetic, same order: bitwise the rows of k_build_rows.
+// Same geometry (kernel_eval.cuh) and the channel loop in the same order: bitwise the rows of k_build_rows.
 template <int MODE, int NC4>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32)
 k_build_rows_voxel(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ xyz, const int32_t* __restrict__ range,
@@ -109,26 +107,21 @@ k_build_rows_voxel(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ x
   }
   int dx, dy, dz;
   slot_to_d(lane < 27 ? lane : 13, dx, dy, dz);
-  const int off = level_offset(l);
+  const double cx = voxel_centre(ux, l), cy = voxel_centre(uy, l), cz = voxel_centre(uz, l);
   const double inv = (1.0 / (double)svh.voxel_size) * (1.0 / (double)(1 << l));
-  const double cx = (double)(ux - off) + 0.5, cy = (double)(uy - off) + 0.5, cz = (double)(uz - off) + 0.5;
   const float iw = 1.f / (svh.voxel_size * (float)(1 << l));
   const int L = svh.depth;
   for (int q = r.x; q < r.y; ++q) {
     const float px = __ldg(xyz + 3 * (int64_t)q), py = __ldg(xyz + 3 * (int64_t)q + 1), pz = __ldg(xyz + 3 * (int64_t)q + 2);
-    const float tx = (float)((double)px * inv - cx), ty = (float)((double)py * inv - cy),
-                tz = (float)((double)pz * inv - cz);
-    float bx, dbx, ttx, dtx, by, dby, tty, dty, bz, dbz, ttz, dtz;
-    axis_weights(tx, dx, bx, dbx, ttx, dtx);
-    axis_weights(ty, dy, by, dby, tty, dty);
-    axis_weights(tz, dz, bz, dbz, ttz, dtz);
-    const float B3 = bx * by * bz;
-    const float T3 = ok ? ttx * tty * ttz : 0.f;
+    const float tx = local_coord(px, inv, cx), ty = local_coord(py, inv, cy), tz = local_coord(pz, inv, cz);
+    const StencilWeights w = stencil_weights(tx, ty, tz, dx, dy, dz);
+    const float B3 = w.B3();
+    const float T3 = ok ? w.T3() : 0.f;
     float dT3[3] = {0.f, 0.f, 0.f};
     if (GRAD) {
-      dT3[0] = ok ? dtx * tty * ttz : 0.f;
-      dT3[1] = ok ? ttx * dty * ttz : 0.f;
-      dT3[2] = ok ? ttx * tty * dtz : 0.f;
+      dT3[0] = ok ? w.dT3(0) : 0.f;
+      dT3[1] = ok ? w.dT3(1) : 0.f;
+      dT3[2] = ok ? w.dT3(2) : 0.f;
     }
     float dot = 0.f, ddot[3] = {0.f, 0.f, 0.f};
 #pragma unroll
@@ -145,9 +138,9 @@ k_build_rows_voxel(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ x
     }
     float* out = e + ((int64_t)q * L + l) * ROWS * NKSR_ROW_STRIDE;
     if (GRAD) {
-      out[lane] = ok ? (dbx * by * bz * dot + B3 * ddot[0]) * iw : 0.f;
-      out[32 + lane] = ok ? (bx * dby * bz * dot + B3 * ddot[1]) * iw : 0.f;
-      out[64 + lane] = ok ? (bx * by * dbz * dot + B3 * ddot[2]) * iw : 0.f;
+      out[lane] = ok ? (w.dB(0) * dot + B3 * ddot[0]) * iw : 0.f;
+      out[32 + lane] = ok ? (w.dB(1) * dot + B3 * ddot[1]) * iw : 0.f;
+      out[64 + lane] = ok ? (w.dB(2) * dot + B3 * ddot[2]) * iw : 0.f;
     } else if (MODE == 2) {
       const float tau = lane == 27 ? tx : (lane == 28 ? ty : tz);
       out[lane] = lane < 27 ? (ok ? dot : 0.f) : (lane < 30 ? tau : 0.f);
@@ -182,29 +175,19 @@ k_evaluate(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ alpha, co
   const int64_t i = blockIdx.x * (int64_t)kWarpsPerBlock + (threadIdx.x >> 5);
   if (i >= m) return;
   const float px = __ldg(xyz + 3 * i), py = __ldg(xyz + 3 * i + 1), pz = __ldg(xyz + 3 * i + 2);
-  const float half_w = svh.voxel_size * 0.5f;
-  int u[3];
-  bool bad = false;
-  {
-    float p[3] = {px, py, pz};
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-      float q = floorf(__fdiv_rn(p[a], half_w));
-      if (!(q > -(float)(NKSR_HALF_OFFSET - 16) && q < (float)(NKSR_HALF_OFFSET - 16))) { bad = true; q = 0.f; }
-      u[a] = (int)q + NKSR_HALF_OFFSET;
-    }
-  }
+  int3 h;
+  const bool in_range = half_voxel(px, py, pz, svh.voxel_size * 0.5f, h);
   const int L = svh.depth;
   const double inv0 = 1.0 / (double)svh.voxel_size;
   int idx = -1;
-  if (!bad && svh.n[L - 1] > 0)
-    idx = find_key(svh.keys[L - 1], svh.n[L - 1], morton3(u[0] >> L, u[1] >> L, u[2] >> L));
+  if (in_range && svh.n[L - 1] > 0)
+    idx = find_key(svh.keys[L - 1], svh.n[L - 1], morton3(h.x >> L, h.y >> L, h.z >> L));
   float accf = 0.f, accg[3] = {0.f, 0.f, 0.f};
   for (int l = L - 1; l >= 0; --l) {
     if (idx < 0) break;  // parent closure: nothing active below
     const float wl = svh.voxel_size * (float)(1 << l);
     LaneKernel r = eval_level_lane<GRAD>(svh.nbr27[l], feat.z[l], feat.channels, l, wl, inv0, px, py, pz, idx,
-                                         u[0] >> (l + 1), u[1] >> (l + 1), u[2] >> (l + 1), fullgrad, lane);
+                                         h.x >> (l + 1), h.y >> (l + 1), h.z >> (l + 1), fullgrad, lane);
     float a = r.nb >= 0 ? __ldg(alpha + svh.offset[l] + r.nb) : 0.f;
     accf = fmaf(a, r.k, accf);
     if (GRAD) {
@@ -212,10 +195,7 @@ k_evaluate(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ alpha, co
       accg[1] = fmaf(a, r.dk[1], accg[1]);
       accg[2] = fmaf(a, r.dk[2], accg[2]);
     }
-    if (l > 0) {
-      int slot = (((u[0] >> l) & 1) << 2) | (((u[1] >> l) & 1) << 1) | ((u[2] >> l) & 1);
-      idx = __ldg(svh.child8[l] + (int64_t)idx * 8 + slot);
-    }
+    if (l > 0) idx = __ldg(svh.child8[l] + (int64_t)idx * 8 + child_octant(h, l));
   }
   accf = warp_sum(accf);
   if (GRAD) {
@@ -233,8 +213,8 @@ k_evaluate(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ alpha, co
 // consecutive queries share their containing voxel on the coarse levels almost always and on the finest level about
 // half of the time.  One warp walks kEvalRun consecutive queries and keeps, per level, the containing voxel with its
 // 27 neighbours, their features (one float4) and coefficients in registers; a level is re-fetched only when the
-// query leaves the voxel.  k_evaluate re-gathers all of it per query and level (three 27-wavefront gathers each).  Same arithmetic in the same order: bitwise the values of
-// k_evaluate<false>.
+// query leaves the voxel.  k_evaluate re-gathers all of it per query and level (three 27-wavefront gathers each).  Same geometry
+// (kernel_eval.cuh) and the channel loop in the same order: bitwise the values of k_evaluate<false>.
 constexpr int kEvalRun = 8;
 constexpr int kEvalMaxL = 4;
 
@@ -261,32 +241,22 @@ k_evaluate_runs(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ alph
   const int64_t q1 = q0 + kEvalRun < m ? q0 + kEvalRun : m;
   for (int64_t i = q0; i < q1; ++i) {
     const float px = __ldg(xyz + 3 * i), py = __ldg(xyz + 3 * i + 1), pz = __ldg(xyz + 3 * i + 2);
-    int u[3];
-    bool bad = false;
-    {
-      const float p[3] = {px, py, pz};
-#pragma unroll
-      for (int a = 0; a < 3; ++a) {
-        float q = floorf(__fdiv_rn(p[a], half_w));
-        if (!(q > -(float)(NKSR_HALF_OFFSET - 16) && q < (float)(NKSR_HALF_OFFSET - 16))) { bad = true; q = 0.f; }
-        u[a] = (int)q + NKSR_HALF_OFFSET;
-      }
-    }
+    int3 h;
+    const bool in_range = half_voxel(px, py, pz, half_w, h);
     float accf = 0.f;
     int idx = -1;
-    bool alive = !bad && svh.n[L - 1] > 0;
+    bool alive = in_range && svh.n[L - 1] > 0;
 #pragma unroll
     for (int ll = 0; ll < kEvalMaxL; ++ll) {
       const int l = L - 1 - ll;                    // coarse to fine
       if (l < 0 || !alive) continue;
-      const int vx = u[0] >> (l + 1), vy = u[1] >> (l + 1), vz = u[2] >> (l + 1);
+      const int vx = h.x >> (l + 1), vy = h.y >> (l + 1), vz = h.z >> (l + 1);
       if (vx != cux[ll] || vy != cuy[ll] || vz != cuz[ll]) {   // left the voxel on this level: re-fetch it
         int nidx;
         if (l == L - 1) {
           nidx = find_key(svh.keys[l], svh.n[l], morton3(vx, vy, vz));
         } else {
-          const int slot = (((u[0] >> (l + 1)) & 1) << 2) | (((u[1] >> (l + 1)) & 1) << 1) | ((u[2] >> (l + 1)) & 1);
-          nidx = idx >= 0 ? __ldg(svh.child8[l + 1] + (int64_t)idx * 8 + slot) : -1;
+          nidx = idx >= 0 ? __ldg(svh.child8[l + 1] + (int64_t)idx * 8 + child_octant(h, l + 1)) : -1;
         }
         cux[ll] = vx; cuy[ll] = vy; cuz[ll] = vz; cidx[ll] = nidx;
         cnb[ll] = -1; ca[ll] = 0.f; cz[ll] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -301,19 +271,13 @@ k_evaluate_runs(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ alph
       }
       idx = cidx[ll];
       if (idx < 0) { alive = false; continue; }   // parent closure: nothing active below
-      // ---- K_l(x, nb) exactly as eval_level_lane<false> computes it
-      const int off = level_offset(l);
       const double inv = inv0 * (1.0 / (double)(1 << l));
-      const float tx = (float)((double)px * inv - ((double)(vx - off) + 0.5));
-      const float ty = (float)((double)py * inv - ((double)(vy - off) + 0.5));
-      const float tz = (float)((double)pz * inv - ((double)(vz - off) + 0.5));
-      float bx, dbx, ttx, dtx, by, dby, tty, dty, bz, dbz, ttz, dtz;
-      axis_weights(tx, dx, bx, dbx, ttx, dtx);
-      axis_weights(ty, dy, by, dby, tty, dty);
-      axis_weights(tz, dz, bz, dbz, ttz, dtz);
+      const StencilWeights w =
+          stencil_weights(local_coord(px, inv, voxel_centre(vx, l)), local_coord(py, inv, voxel_centre(vy, l)),
+                          local_coord(pz, inv, voxel_centre(vz, l)), dx, dy, dz);
       const bool ok = cnb[ll] >= 0;
-      const float B3 = bx * by * bz;
-      const float T3 = ok ? ttx * tty * ttz : 0.f;
+      const float B3 = w.B3();
+      const float T3 = ok ? w.T3() : 0.f;
       float dot = 0.f;
       const float zc[4] = {cz[ll].x, cz[ll].y, cz[ll].z, cz[ll].w};
 #pragma unroll
@@ -334,22 +298,14 @@ __global__ void k_layer_mask(nksr_svh_t svh, const float* __restrict__ xyz, int6
                              float* __restrict__ out) {
   int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= m) return;
-  const float half_w = svh.voxel_size * 0.5f;
-  int u[3];
-  bool bad = false;
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    float q = floorf(__fdiv_rn(__ldg(xyz + 3 * i + a), half_w));
-    if (!(q > -(float)(NKSR_HALF_OFFSET - 16) && q < (float)(NKSR_HALF_OFFSET - 16))) { bad = true; q = 0.f; }
-    u[a] = (int)q + NKSR_HALF_OFFSET;
-  }
+  int3 h;
   float r = 0.f;
-  if (!bad) {
+  if (half_voxel(__ldg(xyz + 3 * i), __ldg(xyz + 3 * i + 1), __ldg(xyz + 3 * i + 2), svh.voxel_size * 0.5f, h)) {
     int top = adaptive_depth < svh.depth ? adaptive_depth : svh.depth;
     for (int l = 0; l < top; ++l) {
       if (svh.n[l] == 0) continue;
       int sh = l + 1;
-      if (find_key(svh.keys[l], svh.n[l], morton3(u[0] >> sh, u[1] >> sh, u[2] >> sh)) >= 0) { r = 1.f; break; }
+      if (find_key(svh.keys[l], svh.n[l], morton3(h.x >> sh, h.y >> sh, h.z >> sh)) >= 0) { r = 1.f; break; }
     }
   }
   out[i] = r;

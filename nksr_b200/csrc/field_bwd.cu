@@ -3,9 +3,10 @@
 //
 // Deterministic by construction, no floating-point atomics: the locations are Morton sorted, so the locations whose
 // level-l stencil contains voxel v are the contiguous ranges (nksr_row_ranges) of v's 27 neighbours u.  Pass 1 (one
-// warp per location, lane = stencil slot, the arithmetic of eval_level_lane) forms the per-(location, level) vectors
-// phi, dphi_a, psi, psi0, psi_a once; pass 2 (one warp per voxel, lane = channel) gathers them over the 27 ranges in
-// slot order and range order, so every output is summed in one fixed order.
+// warp per location, lane = stencil slot) forms the per-(location, level) vectors phi, dphi_a, psi, psi0, psi_a once;
+// pass 2 (one warp per voxel, lane = channel) gathers them over the 27 ranges in slot order and range order, so every
+// output is summed in one fixed order.  Both passes take the kernel's geometry from kernel_eval.cuh, as the forward
+// does.
 #include "kernel_eval.cuh"
 
 namespace {
@@ -43,35 +44,29 @@ k_field_bwd_pass1(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ xy
       for (int a = 0; a < ncf; ++a) cf[k][a] = __ldg(coef + (i * nvec + k) * ncf + a);
   }
   const float px = __ldg(xyz + 3 * i), py = __ldg(xyz + 3 * i + 1), pz = __ldg(xyz + 3 * i + 2);
-  const float half_w = svh.voxel_size * 0.5f;
-  const int hx = (int)floorf(__fdiv_rn(px, half_w)) + NKSR_HALF_OFFSET;
-  const int hy = (int)floorf(__fdiv_rn(py, half_w)) + NKSR_HALF_OFFSET;
-  const int hz = (int)floorf(__fdiv_rn(pz, half_w)) + NKSR_HALF_OFFSET;
+  // a location outside the range has base -1 on every level (nksr_locate), so its h is never read
+  int3 h;
+  half_voxel(px, py, pz, svh.voxel_size * 0.5f, h);
   const double inv0 = 1.0 / (double)svh.voxel_size;
   int dx, dy, dz;
   slot_to_d(lane < 27 ? lane : 13, dx, dy, dz);
   for (int l = 0; l < L; ++l) {
     const int b = __ldg(base + (int64_t)l * m + i);
     if (b < 0) continue;                               // pass 2 never reads this record
-    const int off = level_offset(l);
     const double inv = inv0 * (1.0 / (double)(1 << l));
-    const float tx = (float)((double)px * inv - ((double)((hx >> (l + 1)) - off) + 0.5));
-    const float ty = (float)((double)py * inv - ((double)((hy >> (l + 1)) - off) + 0.5));
-    const float tz = (float)((double)pz * inv - ((double)((hz >> (l + 1)) - off) + 0.5));
-    float bx, dbx, ttx, dtx, by, dby, tty, dty, bz, dbz, ttz, dtz;
-    axis_weights(tx, dx, bx, dbx, ttx, dtx);
-    axis_weights(ty, dy, by, dby, tty, dty);
-    axis_weights(tz, dz, bz, dbz, ttz, dtz);
+    const StencilWeights w = stencil_weights(local_coord(px, inv, voxel_centre(h.x >> (l + 1), l)),
+                                             local_coord(py, inv, voxel_centre(h.y >> (l + 1), l)),
+                                             local_coord(pz, inv, voxel_centre(h.z >> (l + 1), l)), dx, dy, dz);
     const int nb = lane < 27 ? __ldg(svh.nbr27[l] + (int64_t)b * 27 + lane) : -1;
     const bool ok = nb >= 0;
     const float iw = 1.f / (svh.voxel_size * (float)(1 << l));
-    const float B3 = bx * by * bz;
-    const float T3 = ok ? ttx * tty * ttz : 0.f;
+    const float B3 = w.B3();
+    const float T3 = ok ? w.T3() : 0.f;
     float dT3[3] = {0.f, 0.f, 0.f};
     if (full) {
-      dT3[0] = ok ? dtx * tty * ttz : 0.f;
-      dT3[1] = ok ? ttx * dty * ttz : 0.f;
-      dT3[2] = ok ? ttx * tty * dtz : 0.f;
+      dT3[0] = ok ? w.dT3(0) : 0.f;
+      dT3[1] = ok ? w.dT3(1) : 0.f;
+      dT3[2] = ok ? w.dT3(2) : 0.f;
     }
     // psi weights of this slot: value rows omega B; gradient rows (sum_a omega_a dB_a) / W (psi0), omega_a B / W (psi_a)
     float wpsi = 0.f, wpsia[3] = {0.f, 0.f, 0.f};
@@ -84,7 +79,7 @@ k_field_bwd_pass1(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ xy
       if (!GRAD) {
         wpsi = om[0] * B3;
       } else {
-        wpsi = (om[0] * (dbx * by * bz) + om[1] * (bx * dby * bz) + om[2] * (bx * by * dbz)) * iw;
+        wpsi = (om[0] * w.dB(0) + om[1] * w.dB(1) + om[2] * w.dB(2)) * iw;
         if (full) {
 #pragma unroll
           for (int a = 0; a < 3; ++a) wpsia[a] = om[a] * B3 * iw;
@@ -117,26 +112,6 @@ k_field_bwd_pass1(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ xy
   }
 }
 
-// geometry of location q in its containing voxel u (offset coords cu) on level l, for the slot at offset d
-struct SlotW {
-  float B, T, dB[3], dT[3];
-};
-__device__ __forceinline__ SlotW slot_weights(float px, float py, float pz, double inv, const double* cu, int dx,
-                                              int dy, int dz) {
-  const float tx = (float)((double)px * inv - cu[0]), ty = (float)((double)py * inv - cu[1]),
-              tz = (float)((double)pz * inv - cu[2]);
-  float bx, dbx, ttx, dtx, by, dby, tty, dty, bz, dbz, ttz, dtz;
-  axis_weights(tx, dx, bx, dbx, ttx, dtx);
-  axis_weights(ty, dy, by, dby, tty, dty);
-  axis_weights(tz, dz, bz, dbz, ttz, dtz);
-  SlotW w;
-  w.B = bx * by * bz;
-  w.T = ttx * tty * ttz;
-  w.dB[0] = dbx * by * bz; w.dB[1] = bx * dby * bz; w.dB[2] = bx * by * dbz;
-  w.dT[0] = dtx * tty * ttz; w.dT[1] = ttx * dty * ttz; w.dT[2] = ttx * tty * dtz;
-  return w;
-}
-
 // pass 2, one warp per voxel v of level l, lane = channel.  Visits the neighbours u of v in slot order; v sits in
 // slot 26 - s' of u's stencil (offset -d(s')); every location of u's range in sorted order.
 //   VJP (dz_v += ...):  value     omega B phi + T psi
@@ -162,7 +137,6 @@ k_field_bwd_pass2(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ xy
     av0 = __ldg(a0 + gv);
     av1 = a1 != nullptr ? __ldg(a1 + gv) : 0.f;
   }
-  const int off = level_offset(l);
   const double inv = (1.0 / (double)svh.voxel_size) * (1.0 / (double)(1 << l));
   const float iw = 1.f / (svh.voxel_size * (float)(1 << l));
   const bool live = lane < C;
@@ -174,13 +148,16 @@ k_field_bwd_pass2(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ xy
     if (r.x >= r.y) continue;
     int ux, uy, uz;
     morton3_decode(__ldg(svh.keys[l] + u), ux, uy, uz);
-    const double cu[3] = {(double)(ux - off) + 0.5, (double)(uy - off) + 0.5, (double)(uz - off) + 0.5};
+    const double cx = voxel_centre(ux, l), cy = voxel_centre(uy, l), cz = voxel_centre(uz, l);
     int dx, dy, dz;
     slot_to_d(26 - s, dx, dy, dz);
     for (int q = r.x; q < r.y; ++q) {
       const float px = __ldg(xyz + 3 * (int64_t)q), py = __ldg(xyz + 3 * (int64_t)q + 1),
                   pz = __ldg(xyz + 3 * (int64_t)q + 2);
-      const SlotW w = slot_weights(px, py, pz, inv, cu, dx, dy, dz);
+      const StencilWeights w =
+          stencil_weights(local_coord(px, inv, cx), local_coord(py, inv, cy), local_coord(pz, inv, cz), dx, dy, dz);
+      const float B3 = w.B3(), T3 = w.T3();
+      const float dB[3] = {w.dB(0), w.dB(1), w.dB(2)}, dT3[3] = {w.dT3(0), w.dT3(1), w.dT3(2)};
       const float* rq = rec + ((int64_t)q * L + l) * nq * C + (live ? lane : 0);
       float om[3];
 #pragma unroll
@@ -197,21 +174,21 @@ k_field_bwd_pass2(nksr_svh_t svh, nksr_feat_t feat, const float* __restrict__ xy
       if (!live) continue;
       const float phi = __ldg(rq);
       if (!GRAD) {
-        acc = fmaf(om[0] * w.B, phi, acc);
-        if (!ADJ) acc = fmaf(w.T, __ldg(rq + C), acc);
+        acc = fmaf(om[0] * B3, phi, acc);
+        if (!ADJ) acc = fmaf(T3, __ldg(rq + C), acc);
       } else {
-        float t = (om[0] * w.dB[0] + om[1] * w.dB[1] + om[2] * w.dB[2]) * phi;
+        float t = (om[0] * dB[0] + om[1] * dB[1] + om[2] * dB[2]) * phi;
         if (full) {
 #pragma unroll
-          for (int a = 0; a < 3; ++a) t = fmaf(om[a] * w.B, __ldg(rq + (1 + a) * C), t);
+          for (int a = 0; a < 3; ++a) t = fmaf(om[a] * B3, __ldg(rq + (1 + a) * C), t);
         }
         acc = fmaf(t, iw, acc);
         if (!ADJ) {
           const int p0 = full ? 4 : 1;                 // psi0, then psi_a
-          acc = fmaf(w.T, __ldg(rq + p0 * C), acc);
+          acc = fmaf(T3, __ldg(rq + p0 * C), acc);
           if (full) {
 #pragma unroll
-            for (int a = 0; a < 3; ++a) acc = fmaf(w.dT[a], __ldg(rq + (p0 + 1 + a) * C), acc);
+            for (int a = 0; a < 3; ++a) acc = fmaf(dT3[a], __ldg(rq + (p0 + 1 + a) * C), acc);
           }
         }
       }

@@ -101,6 +101,34 @@ struct PlaceArg<true> {
   }
 };
 
+// Compact gradient rows (SPEC S4): the quadratic B-spline of stencil offset d as polynomials in tau,
+// b = c0 + tau (c1 + c2 tau), db = c1 + 2 c2 tau.  Not bitwise axis_weights (kernel_eval.cuh), so a separate definition.
+struct CompactSpline {
+  float c0[3], c1[3], c2[3];
+  __device__ __forceinline__ CompactSpline(int dx, int dy, int dz) {
+    const int d[3] = {dx, dy, dz};
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      c0[a] = d[a] == 0 ? 0.75f : 0.125f;
+      c1[a] = 0.5f * (float)d[a];
+      c2[a] = d[a] == 0 ? -1.f : 0.5f;
+    }
+  }
+  // one level's line (<phi,z_s> in lanes 0..26, tau in 27..29) -> this lane's entries of the three gradient rows,
+  // e_a = dB_a B_b B_c <phi,z_s> * iw with iw = 1 / W_level.  All 32 lanes must call.
+  __device__ __forceinline__ void grad_rows(float line, float iw, int lane, float& e0, float& e1, float& e2) const {
+    const float tx = __shfl_sync(0xffffffffu, line, 27), ty = __shfl_sync(0xffffffffu, line, 28),
+                tz = __shfl_sync(0xffffffffu, line, 29);
+    const float bx = fmaf(fmaf(c2[0], tx, c1[0]), tx, c0[0]), dbx = fmaf(2.f * c2[0], tx, c1[0]);
+    const float by = fmaf(fmaf(c2[1], ty, c1[1]), ty, c0[1]), dby = fmaf(2.f * c2[1], ty, c1[1]);
+    const float bz = fmaf(fmaf(c2[2], tz, c1[2]), tz, c0[2]), dbz = fmaf(2.f * c2[2], tz, c1[2]);
+    const float sc = (lane < 27 ? line : 0.f) * iw;
+    e0 = dbx * by * bz * sc;
+    e1 = bx * dby * bz * sc;
+    e2 = bx * by * dbz * sc;
+  }
+};
+
 __device__ __forceinline__ void row_of_warp(const nksr_svh_t& svh, int64_t row, int& l, int& i) {
   l = 0;
   while (l + 1 < svh.depth && row >= svh.offset[l + 1]) ++l;

@@ -207,10 +207,7 @@ k_gram_fill_group(const nksr_svh_t svh, const nksr_feat_t feat, const nksr_const
                 (Ak[2][k - 1] - ((2 * Pz - 1) >> k));
   }
   const bool use_blocks = cs.mblocks != nullptr && l >= cs.split_level;
-  // quadratic B-spline of this lane's offset as polynomials in tau (compact gradient rows, SPEC S4)
-  const float cx0 = ldx == 0 ? 0.75f : 0.125f, cx1 = 0.5f * (float)ldx, cx2 = ldx == 0 ? -1.f : 0.5f;
-  const float cy0 = ldy == 0 ? 0.75f : 0.125f, cy1 = 0.5f * (float)ldy, cy2 = ldy == 0 ? -1.f : 0.5f;
-  const float cz0 = ldz == 0 ? 0.75f : 0.125f, cz1 = 0.5f * (float)ldz, cz2 = ldz == 0 ? -1.f : 0.5f;
+  const CompactSpline spline(ldx, ldy, ldz);
   const float inv_wl = 1.f / (svh.voxel_size * (float)(1 << l));
 
   float R[8][NLEV];
@@ -269,16 +266,7 @@ k_gram_fill_group(const nksr_svh_t svh, const nksr_feat_t feat, const nksr_const
             float iw = inv_wl;
 #pragma unroll
             for (int k = 0; k < NLEV; ++k) {
-              const float line = __ldg(p + k * NKSR_ROW_STRIDE);
-              const float tx = __shfl_sync(0xffffffffu, line, 27), ty = __shfl_sync(0xffffffffu, line, 28),
-                          tz = __shfl_sync(0xffffffffu, line, 29);
-              const float bx = fmaf(fmaf(cx2, tx, cx1), tx, cx0), dbx = fmaf(2.f * cx2, tx, cx1);
-              const float by = fmaf(fmaf(cy2, ty, cy1), ty, cy0), dby = fmaf(2.f * cy2, ty, cy1);
-              const float bz = fmaf(fmaf(cz2, tz, cz1), tz, cz0), dbz = fmaf(2.f * cz2, tz, cz1);
-              const float sc = (lane < 27 ? line : 0.f) * iw;
-              e[0][k] = dbx * by * bz * sc;
-              e[1][k] = bx * dby * bz * sc;
-              e[2][k] = bx * by * dbz * sc;
+              spline.grad_rows(__ldg(p + k * NKSR_ROW_STRIDE), iw, lane, e[0][k], e[1][k], e[2][k]);
               iw *= 0.5f;
             }
             const float* t = cs.t_nrm + (int64_t)q * 3;

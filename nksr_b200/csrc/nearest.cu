@@ -20,14 +20,9 @@ k_nearest_point(const nksr_svh_t svh, const float* __restrict__ xyz, const int32
   const int64_t i = blockIdx.x * (int64_t)kNearWarps + (threadIdx.x >> 5);
   if (i >= m) return;
   const float qx = __ldg(query + 3 * i), qy = __ldg(query + 3 * i + 1), qz = __ldg(query + 3 * i + 2);
-  const float half_w = svh.voxel_size * 0.5f;
   // half-voxel coordinates in the frame of the keys (cloud shifted to its bounding-box corner)
-  const float fx = floorf(__fdiv_rn(qx - ox, half_w)), fy = floorf(__fdiv_rn(qy - oy, half_w)),
-              fz = floorf(__fdiv_rn(qz - oz, half_w));
-  const float lim = (float)(NKSR_HALF_OFFSET - 16);
-  const bool bad = !(fabsf(fx) < lim && fabsf(fy) < lim && fabsf(fz) < lim);
-  const int hx = bad ? 0 : (int)fx + NKSR_HALF_OFFSET, hy = bad ? 0 : (int)fy + NKSR_HALF_OFFSET,
-            hz = bad ? 0 : (int)fz + NKSR_HALF_OFFSET;
+  int3 h;
+  const bool bad = !half_voxel(qx - ox, qy - oy, qz - oz, svh.voxel_size * 0.5f, h);
   const int L = svh.depth;
   int dx, dy, dz;
   slot_to_d(lane < 27 ? lane : 13, dx, dy, dz);
@@ -36,7 +31,7 @@ k_nearest_point(const nksr_svh_t svh, const float* __restrict__ xyz, const int32
   for (int l = start_level < L ? start_level : L - 1; l < L; ++l) {
     int rb = 0, re = 0;
     if (lane < 27 && !bad) {
-      const int cx = (hx >> (l + 1)) + dx, cy = (hy >> (l + 1)) + dy, cz = (hz >> (l + 1)) + dz;
+      const int cx = (h.x >> (l + 1)) + dx, cy = (h.y >> (l + 1)) + dy, cz = (h.z >> (l + 1)) + dz;
       if (cx >= 0 && cy >= 0 && cz >= 0) {
         const int v = find_key(svh.keys[l], svh.n[l], morton3(cx, cy, cz));
         if (v >= 0) {

@@ -21,23 +21,19 @@ __device__ __forceinline__ int knn_query(const nksr_svh_t& svh, const float* __r
                                          const float oy, const float oz, const int start_level, const int k,
                                          const float qx, const float qy, const float qz,
                                          unsigned long long* __restrict__ key, const int lane) {
-  const float half_w = svh.voxel_size * 0.5f;
-  const float fx = floorf(__fdiv_rn(qx - ox, half_w)), fy = floorf(__fdiv_rn(qy - oy, half_w)),
-              fz = floorf(__fdiv_rn(qz - oz, half_w));
-  const float lim = (float)(NKSR_HALF_OFFSET - 16);
-  const bool bad = !(fabsf(fx) < lim && fabsf(fy) < lim && fabsf(fz) < lim);
-  const int hx = bad ? 0 : (int)fx + NKSR_HALF_OFFSET, hy = bad ? 0 : (int)fy + NKSR_HALF_OFFSET,
-            hz = bad ? 0 : (int)fz + NKSR_HALF_OFFSET;
+  int3 h;
+  const bool bad = !half_voxel(qx - ox, qy - oy, qz - oz, svh.voxel_size * 0.5f, h);
   const int L = svh.depth;
   int dx, dy, dz;
   slot_to_d(lane < 27 ? lane : 13, dx, dy, dz);
   int fill = 0, got = 0;
   float bound = 3.0e38f, dk2 = 0.f;
   bool exact = false;
-  for (int l = start_level < L ? start_level : L - 1; l < L && !bad; ++l) {
+  // out of range: no level search, only the scan of the whole cloud below
+  for (int l = bad ? L : (start_level < L ? start_level : L - 1); l < L; ++l) {
     int rb = 0, re = 0;
     if (lane < 27) {
-      const int cx = (hx >> (l + 1)) + dx, cy = (hy >> (l + 1)) + dy, cz = (hz >> (l + 1)) + dz;
+      const int cx = (h.x >> (l + 1)) + dx, cy = (h.y >> (l + 1)) + dy, cz = (h.z >> (l + 1)) + dz;
       if (cx >= 0 && cy >= 0 && cz >= 0) {
         const int v = find_key(svh.keys[l], svh.n[l], morton3(cx, cy, cz));
         if (v >= 0) {

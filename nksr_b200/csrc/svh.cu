@@ -12,19 +12,9 @@ __global__ void k_point_half_keys(const float* __restrict__ xyz, int64_t n, floa
                                   int64_t* __restrict__ keys, int32_t* __restrict__ status) {
   int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
-  int u[3];
-  bool bad = false;
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    float q = floorf(__fdiv_rn(__ldg(xyz + 3 * i + a), half_w));  // IEEE division: SPEC S1
-    if (!(q > -(float)(NKSR_HALF_OFFSET - 16) && q < (float)(NKSR_HALF_OFFSET - 16))) {
-      bad = true;
-      q = 0.f;
-    }
-    u[a] = (int)q + NKSR_HALF_OFFSET;
-  }
-  if (bad) atomicOr(status, 1);
-  keys[i] = morton3(u[0], u[1], u[2]);
+  int3 h;
+  if (!half_voxel(__ldg(xyz + 3 * i), __ldg(xyz + 3 * i + 1), __ldg(xyz + 3 * i + 2), half_w, h)) atomicOr(status, 1);
+  keys[i] = morton3(h.x, h.y, h.z);
 }
 
 struct ShiftOp {
@@ -128,25 +118,14 @@ __global__ void k_locate(nksr_svh_t svh, const float* __restrict__ xyz, int64_t 
                          int32_t* __restrict__ base) {
   int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= m) return;
-  int u[3];
-  bool bad = false;
-#pragma unroll
-  for (int a = 0; a < 3; ++a) {
-    float q = floorf(__fdiv_rn(__ldg(xyz + 3 * i + a), half_w));
-    if (!(q > -(float)(NKSR_HALF_OFFSET - 16) && q < (float)(NKSR_HALF_OFFSET - 16))) { bad = true; q = 0.f; }
-    u[a] = (int)q + NKSR_HALF_OFFSET;
-  }
+  int3 h;
+  const bool ok = half_voxel(__ldg(xyz + 3 * i), __ldg(xyz + 3 * i + 1), __ldg(xyz + 3 * i + 2), half_w, h);
   const int L = svh.depth;
   int idx = -1;
-  if (!bad && svh.n[L - 1] > 0)
-    idx = find_key(svh.keys[L - 1], svh.n[L - 1], morton3(u[0] >> L, u[1] >> L, u[2] >> L));
+  if (ok && svh.n[L - 1] > 0) idx = find_key(svh.keys[L - 1], svh.n[L - 1], morton3(h.x >> L, h.y >> L, h.z >> L));
   base[(int64_t)(L - 1) * m + i] = idx;
   for (int l = L - 2; l >= 0; --l) {
-    if (idx >= 0) {
-      int sh = l + 1;
-      int slot = (((u[0] >> sh) & 1) << 2) | (((u[1] >> sh) & 1) << 1) | ((u[2] >> sh) & 1);
-      idx = __ldg(svh.child8[l + 1] + (int64_t)idx * 8 + slot);
-    }
+    if (idx >= 0) idx = __ldg(svh.child8[l + 1] + (int64_t)idx * 8 + child_octant(h, l + 1));
     base[(int64_t)l * m + i] = idx;
   }
 }
