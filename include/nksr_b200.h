@@ -144,10 +144,8 @@ NKSR_API int nksr_build_rows(const nksr_svh_t* svh, const nksr_feat_t* feat, con
 NKSR_API int nksr_build_rows_voxel(const nksr_svh_t* svh, const nksr_feat_t* feat, const float* xyz,
                           const int32_t* base, const int32_t* range, int64_t m, int mode, int approx_kernel_grad,
                           float* e, void* stream);
-/* structural row lengths of A: cnt[i] (same + coarser levels), cnt_down[i] (finer levels) */
-NKSR_API int nksr_gram_count(const nksr_svh_t* svh, int32_t* cnt, int32_t* cnt_down, void* stream);
 NKSR_API size_t nksr_scan_workspace_bytes(int64_t n);
-/* rowptr[0..n] (int64) = exclusive scan of cnt[i] + cnt_down[i] */
+/* rowptr[0..n] (int64) = exclusive scan of cnt[i] (same + coarser levels) + cnt_down[i] (finer levels, nksr_gram_place) */
 NKSR_API int nksr_gram_rowptr(const int32_t* cnt, const int32_t* cnt_down, int64_t n, int64_t* rowptr,
                      void* ws, size_t ws_bytes, void* stream);
 typedef struct {
@@ -176,16 +174,8 @@ NKSR_API int64_t nksr_gram_block_floats(const nksr_svh_t* svh, int split_level);
  * c->split_level must be set; c->mblocks is ignored here) */
 NKSR_API int nksr_gram_blocks(const nksr_svh_t* svh, const nksr_constraints_t* c, float* mblocks,
                      void* stream);
-/* numeric assembly: fills col/val (CSR, int64 rowptr), rhs b, diag. cursor[n] must be zero. */
-NKSR_API int nksr_gram_fill(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
-                   const int32_t* cnt, const int64_t* rowptr, int32_t* col, float* val,
-                   float* rhs, float* diag, int32_t* cursor, void* stream);
-/* sort the finer-level (transposed) segment of every row by column: deterministic storage */
-NKSR_API int nksr_gram_sort_down(const int32_t* cnt, const int32_t* cnt_down, const int64_t* rowptr,
-                        const int32_t* rows, int64_t n_rows, int cap, int32_t* col, float* val,
-                        void* stream);
 
-/* -- sort-free placement of the transposed entries (DESIGN.md SPEC S6b): same matrix, no atomics, no sort.
+/* -- sort-free placement of the transposed entries (DESIGN.md SPEC S6b): no atomics, no sort.
  * Fine voxel j (level l) reaches coarse voxel c (level l+k) through its ancestor a = c - d; its entry sits at
  *   rowptr[c] + cnt[c] + prefix[l][k][c*125 + slot(d)] + rank8[l][k][j*8 + S(d)],  S(d) = axes with |d| = 2. */
 typedef struct {
@@ -199,7 +189,8 @@ NKSR_API int nksr_gram_count_own(const nksr_svh_t* svh, int32_t* cnt, void* stre
  * cnt_down must start at zero and, for one coarse level, the pairs must be issued in increasing l. */
 NKSR_API int nksr_gram_place(const nksr_svh_t* svh, int l, int k, int32_t* rank8, int32_t* class_count,
                     int32_t* prefix, int32_t* cnt_down, void* stream);
-/* nksr_gram_fill with the transposed copies written at their final position */
+/* numeric assembly, one warp per matrix row: fills col/val (CSR, int64 rowptr, row lengths cnt from
+ * nksr_gram_count_own / nksr_gram_count_grouped), rhs b and diag; the transposed copies go to their final position */
 NKSR_API int nksr_gram_fill_placed(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
                           const int32_t* cnt, const int64_t* rowptr, const nksr_placement_t* placement,
                           int32_t* col, float* val, float* rhs, float* diag, void* stream);

@@ -71,13 +71,10 @@ _SIGNATURES = {
     "nksr_transpose_taps": ("i", "pqiqppp"),
     "nksr_build_rows": ("i", "SFppqiipp"),
     "nksr_build_rows_voxel": ("i", "SFpppqiipp"),
-    "nksr_gram_count": ("i", "Sppp"),
     "nksr_scan_workspace_bytes": ("z", "q"),
     "nksr_gram_rowptr": ("i", "ppqppzp"),
-    "nksr_gram_fill": ("i", "SFKppppppp" + "p"),
     "nksr_gram_block_floats": ("q", "Si"),
     "nksr_gram_blocks": ("i", "SKpp"),
-    "nksr_gram_sort_down": ("i", "ppppqippp"),
     "nksr_gram_count_own": ("i", "Spp"),
     "nksr_gram_place": ("i", "Siipppp" + "p"),
     "nksr_gram_fill_placed": ("i", "SFKppPppppp"),

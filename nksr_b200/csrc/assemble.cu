@@ -5,8 +5,8 @@
 // Layout (DESIGN.md SPEC S6): unknowns are ordered level-major, Morton inside a level.  Row
 // (l,i) stores, in this order, [same-level 125-stencil | coarser level l+1 (<=64) | ... | level
 // L-1 | finer-level entries (transposes)].  Only ACTIVE column voxels are stored.  The transposed copies
-// go straight to their final slot from two prefix tables (k_place_rank / k_place_prefix, SPEC S6b); the
-// older atomic-cursor + segment-sort variant is kept behind solver_config['placement'] = 'sorted'.
+// go straight to their final slot from two prefix tables (k_place_rank / k_place_prefix, SPEC S6b): no
+// atomics and no sort, the same storage order on every run.
 //
 // Numeric phase: one warp per row.  For each of the 27 voxels u around i, the constraint rows
 // whose containing voxel is u form one contiguous range (locations are Morton sorted); every
@@ -29,10 +29,9 @@
 
 namespace {
 
-// DOWN = false: own entries only (the transposed segments are sized by k_place_prefix)
-template <bool DOWN>
+// own entries only (the transposed segments are sized by k_place_prefix)
 __global__ void __launch_bounds__(kWarps * 32)
-k_gram_count(nksr_svh_t svh, int64_t n_total, int32_t* __restrict__ cnt, int32_t* __restrict__ cnt_down) {
+k_gram_count(nksr_svh_t svh, int64_t n_total, int32_t* __restrict__ cnt) {
   const int lane = threadIdx.x & 31;
   const int64_t row = blockIdx.x * (int64_t)kWarps + (threadIdx.x >> 5);
   if (row >= n_total) return;
@@ -45,7 +44,6 @@ k_gram_count(nksr_svh_t svh, int64_t n_total, int32_t* __restrict__ cnt, int32_t
   for (int t0 = 0; t0 < nslots; t0 += 32) {
     int t = t0 + lane, k = 0;
     int col = t < nslots ? slot_column(svh, l, g, t, k) : -1;
-    if (DOWN && col >= 0 && k > 0) atomicAdd(cnt_down + svh.offset[l + k] + col, 1);
     c += __popc(__ballot_sync(0xffffffffu, col >= 0));
   }
   if (lane == 0) cnt[row] = c;
@@ -273,12 +271,12 @@ k_gram_blocks(nksr_svh_t svh, nksr_constraints_t cs, float* __restrict__ mblocks
 // (value rows) or of one axis of it (gradient rows): 1 + 3 wide loads per visited location instead of 4 + 12 narrow ones
 // (with narrow loads the LSU was the busiest unit of the kernel).  Same products in the same order: the matrix is
 // bitwise the one of the plain layout.
-template <bool COMPACT, int MAXL, int MINB, bool PLACED, bool ILV>
+template <bool COMPACT, int MAXL, int MINB, bool ILV>
 __global__ void __launch_bounds__(kWarps * 32, MINB)
 k_gram_fill(nksr_svh_t svh, nksr_feat_t feat, nksr_constraints_t cs, int64_t row_begin, int64_t row_end,
             const int32_t* __restrict__ cnt, const int64_t* __restrict__ rowptr, int32_t* __restrict__ col_out,
             float* __restrict__ val_out, float* __restrict__ rhs, float* __restrict__ diag,
-            int32_t* __restrict__ cursor, const PlaceArg<PLACED> place) {
+            const nksr_placement_t place) {
   extern __shared__ float smem[];
   const int lane = threadIdx.x & 31;
   const int wid = threadIdx.x >> 5;
@@ -474,115 +472,8 @@ k_gram_fill(nksr_svh_t svh, nksr_feat_t feat, nksr_constraints_t cs, int64_t row
   }
   gram_row_regulariser(feat, cs, l, i, my_u, lane, acc);
   __syncwarp();
-  gram_row_writeout<MAXL, PLACED>(svh, l, i, row, g, acc, cnt, rowptr, col_out, val_out, diag, cursor, place, lane);
+  gram_row_writeout<MAXL>(svh, l, i, row, g, acc, cnt, rowptr, col_out, val_out, diag, place, lane);
   if (lane == 0) rhs[row] = bsum;
-}
-
-// Sort of the finer-level (transposed) segment of each listed row by column.  (column, value)
-// pairs are packed into one 64-bit word (column in the high half) so a compare-exchange is one
-// 8-byte shared-memory access per side; every thread owns a compare-exchange pair (no idle half).
-__global__ void k_sort_down(const int32_t* __restrict__ cnt, const int32_t* __restrict__ cnt_down,
-                            const int64_t* __restrict__ rowptr, const int32_t* __restrict__ rows, int64_t n_rows,
-                            int32_t* __restrict__ col, float* __restrict__ val, int cap) {
-  extern __shared__ unsigned long long skey[];
-  if (blockIdx.x >= n_rows) return;
-  const int64_t row = rows[blockIdx.x];
-  const int m = cnt_down[row];
-  if (m <= 1 || m > cap) return;
-  const int64_t p0 = rowptr[row] + cnt[row];
-  int m2 = 1;
-  while (m2 < m) m2 <<= 1;
-  for (int t = threadIdx.x; t < m2; t += blockDim.x)
-    skey[t] = t < m ? (((unsigned long long)(unsigned)col[p0 + t] << 32) | __float_as_uint(val[p0 + t]))
-                    : 0xffffffffffffffffull;
-  __syncthreads();
-  const int half = m2 >> 1;
-  for (int k = 2; k <= m2; k <<= 1) {
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int q = threadIdx.x; q < half; q += blockDim.x) {
-        const int lo = ((q & ~(j - 1)) << 1) | (q & (j - 1));
-        const int hi = lo | j;
-        const unsigned long long a = skey[lo], b = skey[hi];
-        if ((a > b) == ((lo & k) == 0)) { skey[lo] = b; skey[hi] = a; }
-      }
-      __syncthreads();
-    }
-  }
-  for (int t = threadIdx.x; t < m; t += blockDim.x) {
-    const unsigned long long v = skey[t];
-    col[p0 + t] = (int32_t)(v >> 32);
-    val[p0 + t] = __uint_as_float((unsigned)v);
-  }
-}
-
-// segments of 33..512 entries: one WARP per row on its own shared-memory tile; stages are separated
-// by __syncwarp only, and eight rows share a block (8x fewer blocks than a block per row)
-template <int CAP>
-__global__ void __launch_bounds__(256)
-k_sort_down_tile(const int32_t* __restrict__ cnt, const int32_t* __restrict__ cnt_down,
-                 const int64_t* __restrict__ rowptr, const int32_t* __restrict__ rows, int64_t n_rows,
-                 int32_t* __restrict__ col, float* __restrict__ val) {
-  __shared__ unsigned long long tile[8][CAP];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int64_t r = blockIdx.x * (int64_t)8 + wid;
-  if (r >= n_rows) return;
-  const int64_t row = rows[r];
-  const int m = cnt_down[row];
-  if (m <= 1 || m > CAP) return;
-  unsigned long long* skey = tile[wid];
-  const int64_t p0 = rowptr[row] + cnt[row];
-  int m2 = 32;
-  while (m2 < m) m2 <<= 1;
-  for (int t = lane; t < m2; t += 32)
-    skey[t] = t < m ? (((unsigned long long)(unsigned)col[p0 + t] << 32) | __float_as_uint(val[p0 + t]))
-                    : 0xffffffffffffffffull;
-  __syncwarp();
-  const int half = m2 >> 1;
-  for (int k = 2; k <= m2; k <<= 1) {
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int q = lane; q < half; q += 32) {
-        const int lo = ((q & ~(j - 1)) << 1) | (q & (j - 1));
-        const int hi = lo | j;
-        const unsigned long long a = skey[lo], b = skey[hi];
-        if ((a > b) == ((lo & k) == 0)) { skey[lo] = b; skey[hi] = a; }
-      }
-      __syncwarp();
-    }
-  }
-  for (int t = lane; t < m; t += 32) {
-    const unsigned long long v = skey[t];
-    col[p0 + t] = (int32_t)(v >> 32);
-    val[p0 + t] = __uint_as_float((unsigned)v);
-  }
-}
-
-// segments of at most 32 entries: one warp per row, bitonic network through shuffles
-__global__ void k_sort_down_warp(const int32_t* __restrict__ cnt, const int32_t* __restrict__ cnt_down,
-                                 const int64_t* __restrict__ rowptr, const int32_t* __restrict__ rows,
-                                 int64_t n_rows, int32_t* __restrict__ col, float* __restrict__ val) {
-  const int lane = threadIdx.x & 31;
-  const int64_t r = blockIdx.x * (int64_t)(blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (r >= n_rows) return;
-  const int64_t row = rows[r];
-  const int m = cnt_down[row];
-  if (m <= 1 || m > 32) return;
-  const int64_t p0 = rowptr[row] + cnt[row];
-  unsigned long long key = lane < m ? (((unsigned long long)(unsigned)col[p0 + lane] << 32) |
-                                       __float_as_uint(val[p0 + lane]))
-                                    : 0xffffffffffffffffull;
-#pragma unroll
-  for (int k = 2; k <= 32; k <<= 1) {
-#pragma unroll
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      const unsigned long long other = __shfl_xor_sync(0xffffffffu, key, j);
-      const bool keep_min = ((lane & j) == 0) == ((lane & k) == 0);
-      key = keep_min ? (key < other ? key : other) : (key > other ? key : other);
-    }
-  }
-  if (lane < m) {
-    col[p0 + lane] = (int32_t)(key >> 32);
-    val[p0 + lane] = __uint_as_float((unsigned)key);
-  }
 }
 
 static int64_t total_unknowns(const nksr_svh_t* svh) {
@@ -593,23 +484,12 @@ static int64_t total_unknowns(const nksr_svh_t* svh) {
 
 extern "C" {
 
-int nksr_gram_count(const nksr_svh_t* svh, int32_t* cnt, int32_t* cnt_down, void* stream) {
-  if (!svh || svh->depth < 1 || svh->depth > NKSR_MAX_DEPTH) return NKSR_E_INVALID;
-  if (!svh->nbr125_top && !svh->parent[svh->depth - 1]) return NKSR_E_INVALID;
-  const int64_t n = total_unknowns(svh);
-  if (n == 0) return NKSR_OK;
-  if (cudaMemsetAsync(cnt_down, 0, (size_t)n * sizeof(int32_t), as_stream(stream)) != cudaSuccess) return NKSR_E_CUDA;
-  k_gram_count<true><<<grid_for(n, kWarps), kWarps * 32, 0, as_stream(stream)>>>(*svh, n, cnt, cnt_down);
-  NKSR_CHECK_LAUNCH();
-  return NKSR_OK;
-}
-
 int nksr_gram_count_own(const nksr_svh_t* svh, int32_t* cnt, void* stream) {
   if (!svh || svh->depth < 1 || svh->depth > NKSR_MAX_DEPTH) return NKSR_E_INVALID;
   if (!svh->nbr125_top && !svh->parent[svh->depth - 1]) return NKSR_E_INVALID;
   const int64_t n = total_unknowns(svh);
   if (n == 0) return NKSR_OK;
-  k_gram_count<false><<<grid_for(n, kWarps), kWarps * 32, 0, as_stream(stream)>>>(*svh, n, cnt, nullptr);
+  k_gram_count<<<grid_for(n, kWarps), kWarps * 32, 0, as_stream(stream)>>>(*svh, n, cnt);
   NKSR_CHECK_LAUNCH();
   return NKSR_OK;
 }
@@ -680,14 +560,17 @@ int nksr_gram_blocks(const nksr_svh_t* svh, const nksr_constraints_t* c, float* 
   return NKSR_OK;
 }
 
-}  // extern "C"
+int nksr_gram_fill_placed(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
+                          const int32_t* cnt, const int64_t* rowptr, const nksr_placement_t* placement,
+                          int32_t* col, float* val, float* rhs, float* diag, void* stream) {
+  return nksr_gram_fill_placed_rows(svh, feat, c, cnt, rowptr, placement, 0, -1, col, val, rhs, diag, stream);
+}
 
-namespace {
-template <bool PLACED>
-int launch_fill(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c, const int32_t* cnt,
-                const int64_t* rowptr, int32_t* col, float* val, float* rhs, float* diag, int32_t* cursor,
-                const PlaceArg<PLACED>& place, int64_t row_begin, int64_t row_end, void* stream) {
-  if (!svh || !feat || !c || svh->depth < 1 || svh->depth > NKSR_MAX_DEPTH) return NKSR_E_INVALID;
+int nksr_gram_fill_placed_rows(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
+                               const int32_t* cnt, const int64_t* rowptr, const nksr_placement_t* placement,
+                               int64_t row_begin, int64_t row_end, int32_t* col, float* val, float* rhs, float* diag,
+                               void* stream) {
+  if (!svh || !feat || !c || !placement || svh->depth < 1 || svh->depth > NKSR_MAX_DEPTH) return NKSR_E_INVALID;
   if (!svh->nbr125_top && !svh->parent[svh->depth - 1]) return NKSR_E_INVALID;
   const int64_t n = total_unknowns(svh);
   if (row_end < 0) row_end = n;
@@ -697,8 +580,8 @@ int launch_fill(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_const
   const size_t smem = (size_t)kWarps * kMaxSlots * sizeof(float);
   const int grid = grid_for(row_end - row_begin, kWarps);
 #define NKSR_FILL(COMPACT, MAXL, MINB, ILV)                                                                  \
-  k_gram_fill<COMPACT, MAXL, MINB, PLACED, ILV><<<grid, kWarps * 32, smem, s>>>(                             \
-      *svh, *feat, *c, row_begin, row_end, cnt, rowptr, col, val, rhs, diag, cursor, place)
+  k_gram_fill<COMPACT, MAXL, MINB, ILV><<<grid, kWarps * 32, smem, s>>>(                                     \
+      *svh, *feat, *c, row_begin, row_end, cnt, rowptr, col, val, rhs, diag, *placement)
   // 4 resident blocks per SM (64 registers) for depth <= 4; 5 blocks (48 registers) was measured
   // 1.7x slower (register starvation cuts the loads in flight per warp)
   if (c->nrm_compact == 2) {                          // interleaved rows
@@ -710,59 +593,6 @@ int launch_fill(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_const
     if (c->nrm_compact) NKSR_FILL(true, NKSR_MAX_DEPTH, 2, false); else NKSR_FILL(false, NKSR_MAX_DEPTH, 2, false);
   }
 #undef NKSR_FILL
-  NKSR_CHECK_LAUNCH();
-  return NKSR_OK;
-}
-}  // namespace
-
-extern "C" {
-
-int nksr_gram_fill(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c, const int32_t* cnt,
-                   const int64_t* rowptr, int32_t* col, float* val, float* rhs, float* diag, int32_t* cursor,
-                   void* stream) {
-  if (!cursor) return NKSR_E_INVALID;
-  return launch_fill<false>(svh, feat, c, cnt, rowptr, col, val, rhs, diag, cursor, PlaceArg<false>{}, 0, -1, stream);
-}
-
-int nksr_gram_fill_placed(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
-                          const int32_t* cnt, const int64_t* rowptr, const nksr_placement_t* placement,
-                          int32_t* col, float* val, float* rhs, float* diag, void* stream) {
-  return nksr_gram_fill_placed_rows(svh, feat, c, cnt, rowptr, placement, 0, -1, col, val, rhs, diag, stream);
-}
-
-int nksr_gram_fill_placed_rows(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
-                               const int32_t* cnt, const int64_t* rowptr, const nksr_placement_t* placement,
-                               int64_t row_begin, int64_t row_end, int32_t* col, float* val, float* rhs, float* diag,
-                               void* stream) {
-  if (!placement) return NKSR_E_INVALID;
-  PlaceArg<true> place;
-  place.t = *placement;
-  return launch_fill<true>(svh, feat, c, cnt, rowptr, col, val, rhs, diag, nullptr, place, row_begin, row_end, stream);
-}
-
-int nksr_gram_sort_down(const int32_t* cnt, const int32_t* cnt_down, const int64_t* rowptr, const int32_t* rows,
-                        int64_t n_rows, int cap, int32_t* col, float* val, void* stream) {
-  // one block per listed row; segments longer than `cap` (a power of two <= 16384) are left in
-  // insertion order.
-  if (n_rows <= 0) return NKSR_OK;
-  if (cap < 2 || cap > 16384 || (cap & (cap - 1))) return NKSR_E_INVALID;
-  if (cap * 8 > 48 * 1024 &&
-      cudaFuncSetAttribute(k_sort_down, cudaFuncAttributeMaxDynamicSharedMemorySize, cap * 8) != cudaSuccess)
-    return NKSR_E_CUDA;
-  if (cap <= 32) {
-    k_sort_down_warp<<<grid_for(n_rows, 8), 256, 0, as_stream(stream)>>>(cnt, cnt_down, rowptr, rows, n_rows, col,
-                                                                        val);
-  } else if (cap <= 128) {
-    k_sort_down_tile<128><<<grid_for(n_rows, 8), 256, 0, as_stream(stream)>>>(cnt, cnt_down, rowptr, rows, n_rows,
-                                                                             col, val);
-  } else if (cap <= 512) {
-    k_sort_down_tile<512><<<grid_for(n_rows, 8), 256, 0, as_stream(stream)>>>(cnt, cnt_down, rowptr, rows, n_rows,
-                                                                             col, val);
-  } else {
-    const int threads = cap >= 4096 ? 512 : (cap >= 1024 ? 256 : (cap >= 256 ? 128 : 64));
-    k_sort_down<<<(unsigned)n_rows, threads, cap * 8, as_stream(stream)>>>(cnt, cnt_down, rowptr, rows, n_rows, col,
-                                                                           val, cap);
-  }
   NKSR_CHECK_LAUNCH();
   return NKSR_OK;
 }

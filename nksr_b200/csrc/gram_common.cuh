@@ -88,18 +88,11 @@ __device__ __forceinline__ int slot_column_place(const nksr_svh_t& svh, int l, c
   return c;
 }
 
-// kernel argument of the sort-free placement: empty for the atomic-cursor variant
-template <bool PLACED>
-struct PlaceArg {
-  __device__ __forceinline__ int pos(int, int, int64_t, int, int64_t, int) const { return 0; }
-};
-template <>
-struct PlaceArg<true> {
-  nksr_placement_t t;
-  __device__ __forceinline__ int pos(int l, int k, int64_t c, int ds, int64_t j, int sm) const {
-    return __ldg(t.prefix[l][k] + c * 125 + ds) + __ldg(t.rank8[l][k] + j * 8 + sm);
-  }
-};
+// position of fine voxel j (level l) inside the transposed segment of coarse voxel c (level l+k), from the
+// sort-free placement tables (SPEC S6b)
+__device__ __forceinline__ int placed_pos(const nksr_placement_t& t, int l, int k, int64_t c, int ds, int64_t j, int sm) {
+  return __ldg(t.prefix[l][k] + c * 125 + ds) + __ldg(t.rank8[l][k] + j * 8 + sm);
+}
 
 // Compact gradient rows (SPEC S4): the quadratic B-spline of stencil offset d as polynomials in tau,
 // b = c0 + tau (c1 + c2 tau), db = c1 + 2 c2 tau.  Not bitwise axis_weights (kernel_eval.cuh), so a separate definition.
@@ -155,12 +148,12 @@ __device__ __forceinline__ void gram_row_regulariser(const nksr_feat_t& feat, co
 // (4 chunks of 32), then the 64 slots of every coarser level (2 chunks each) -- the level offset is uniform inside a chunk,
 // so the box bounds, the ancestor and its parent are computed once per level (in the first version a chunk could
 // straddle two levels).  Coarser-level entries also go, transposed, to the coarse row's finer-level segment.
-template <int MAXL, bool PLACED>
+template <int MAXL>
 __device__ __forceinline__ void gram_row_writeout(const nksr_svh_t& svh, int l, int i, int64_t row, const RowGeom& g,
                                                   const float* __restrict__ acc, const int32_t* __restrict__ cnt,
                                                   const int64_t* __restrict__ rowptr, int32_t* __restrict__ col_out,
                                                   float* __restrict__ val_out, float* __restrict__ diag,
-                                                  int32_t* __restrict__ cursor, const PlaceArg<PLACED>& place, int lane) {
+                                                  const nksr_placement_t& place, int lane) {
   const int nup = svh.depth - 1 - l;
   const int64_t p0 = rowptr[row];
   int written = 0;
@@ -174,8 +167,7 @@ __device__ __forceinline__ void gram_row_writeout(const nksr_svh_t& svh, int l, 
       val_out[p] = v;
       if (k == 0 && c == i) diag[row] = v;
       if (k > 0) {  // transposed copy into the coarse row's finer-level segment
-        const int64_t q = rowptr[gc] + cnt[gc] +
-                          (PLACED ? place.pos(l, k, c, ds, i, sm) : atomicAdd(cursor + gc, 1));
+        const int64_t q = rowptr[gc] + cnt[gc] + placed_pos(place, l, k, c, ds, i, sm);
         col_out[q] = (int32_t)row;
         val_out[q] = v;
       }

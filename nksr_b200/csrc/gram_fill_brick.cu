@@ -110,7 +110,7 @@ __global__ void __launch_bounds__(kBrickWarps * 32)
 k_gram_fill_brick(const nksr_svh_t svh, const nksr_feat_t feat, const nksr_constraints_t cs, const int l,
                   const int32_t* __restrict__ cnt, const int64_t* __restrict__ rowptr, int32_t* __restrict__ col_out,
                   float* __restrict__ val_out, float* __restrict__ rhs, float* __restrict__ diag,
-                  const PlaceArg<true> place) {
+                  const nksr_placement_t place) {
   using B = Brick<LB>;
   extern __shared__ __align__(16) float smem[];
   __shared__ unsigned s_starts[2];
@@ -320,7 +320,7 @@ k_gram_fill_brick(const nksr_svh_t svh, const nksr_feat_t feat, const nksr_const
       float* acc = tile + r * ts;
       gram_row_regulariser(feat, cs, l, i, my_u, lane, acc);
       __syncwarp();
-      gram_row_writeout<4, true>(svh, l, i, row, g, acc, cnt, rowptr, col_out, val_out, diag, nullptr, place, lane);
+      gram_row_writeout<4>(svh, l, i, row, g, acc, cnt, rowptr, col_out, val_out, diag, place, lane);
       if (lane == 0) rhs[row] = brhs[r];
     }
     __syncthreads();
@@ -329,7 +329,7 @@ k_gram_fill_brick(const nksr_svh_t svh, const nksr_feat_t feat, const nksr_const
 
 template <int LB, bool ILV>
 int launch_brick_level(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c, int l,
-                       const int32_t* cnt, const int64_t* rowptr, const PlaceArg<true>& place, int32_t* col, float* val,
+                       const int32_t* cnt, const int64_t* rowptr, const nksr_placement_t& place, int32_t* col, float* val,
                        float* rhs, float* diag, cudaStream_t s) {
   const int ts = (125 + 64 * (svh->depth - 1 - l) + 3) & ~3;
   const size_t smem = Brick<LB>::words(ts) * sizeof(float);
@@ -354,8 +354,6 @@ int nksr_gram_fill_brick(const nksr_svh_t* svh, const nksr_feat_t* feat, const n
   // compact gradient rows and hierarchies deeper than 4 levels: the row fill on every row
   const int nb = (c->nrm_compact == 1 || svh->depth > 4) ? 0 : (c->split_level < svh->depth ? c->split_level : svh->depth);
   if (nb < 0) return NKSR_E_INVALID;
-  PlaceArg<true> place;
-  place.t = *placement;
   cudaStream_t s = as_stream(stream);
   const double locations = (double)c->n_pos + (double)c->n_nrm;
   for (int l = 0; l < nb; ++l) {
@@ -368,8 +366,8 @@ int nksr_gram_fill_brick(const nksr_svh_t* svh, const nksr_feat_t* feat, const n
     }
     const int rc =
         c->nrm_compact == 2
-            ? launch_brick_level<kBrickLog2, true>(svh, feat, c, l, cnt, rowptr, place, col, val, rhs, diag, s)
-            : launch_brick_level<kBrickLog2, false>(svh, feat, c, l, cnt, rowptr, place, col, val, rhs, diag, s);
+            ? launch_brick_level<kBrickLog2, true>(svh, feat, c, l, cnt, rowptr, *placement, col, val, rhs, diag, s)
+            : launch_brick_level<kBrickLog2, false>(svh, feat, c, l, cnt, rowptr, *placement, col, val, rhs, diag, s);
     if (rc != NKSR_OK) return rc;
   }
   const int64_t n = svh->offset[svh->depth - 1] + svh->n[svh->depth - 1];

@@ -141,7 +141,7 @@ __global__ void __launch_bounds__(kGW * 32, 4)
 k_gram_fill_group(const nksr_svh_t svh, const nksr_feat_t feat, const nksr_constraints_t cs, const int l,
                   const int32_t* __restrict__ cnt, const int64_t* __restrict__ rowptr,
                   int32_t* __restrict__ col_out, float* __restrict__ val_out, float* __restrict__ rhs,
-                  float* __restrict__ diag, const PlaceArg<true> place) {
+                  float* __restrict__ diag, const nksr_placement_t place) {
   extern __shared__ float smem[];
   const int lane = threadIdx.x & 31;
   const int wid = threadIdx.x >> 5;
@@ -360,7 +360,7 @@ k_gram_fill_group(const nksr_svh_t svh, const nksr_feat_t feat, const nksr_const
         val_out[p] = v;
         if (k == 0 && cv == i) diag[row] = v;
         if (k > 0) {  // transposed copy, straight to its final slot in the coarse row (SPEC S6b)
-          const int64_t q = rowptr[gc] + cnt[gc] + place.pos(l, k, cv, ds, i, sm);
+          const int64_t q = rowptr[gc] + cnt[gc] + placed_pos(place, l, k, cv, ds, i, sm);
           col_out[q] = (int32_t)row;
           val_out[q] = v;
         }
@@ -407,8 +407,6 @@ int nksr_gram_fill_grouped(const nksr_svh_t* svh, const nksr_feat_t* feat, const
   if (svh->depth > 4 || svh->depth >= NKSR_MAX_DEPTH || !svh->parent[svh->depth - 1] || !svh->child8[svh->depth] ||
       !svh->nbr27[svh->depth])
     return NKSR_E_INVALID;
-  PlaceArg<true> place;
-  place.t = *placement;
   cudaStream_t s = as_stream(stream);
   const size_t smem = (size_t)kGW * kWarpWords * sizeof(float);
   const int L = svh->depth;
@@ -423,7 +421,7 @@ int nksr_gram_fill_grouped(const nksr_svh_t* svh, const nksr_feat_t* feat, const
                              (int)smem) != cudaSuccess)                                                       \
       return NKSR_E_CUDA;                                                                                     \
     k_gram_fill_group<NLEV, COMPACT><<<grid, kGW * 32, smem, s>>>(*svh, *feat, *c, l, cnt, rowptr, col, val, rhs, \
-                                                                  diag, place);                               \
+                                                                  diag, *placement);                          \
   } while (0)
     if (c->nrm_compact) {
       switch (nlev) {

@@ -26,10 +26,6 @@ from . import _lib
 from ._lib import call, stream_ptr
 from .svh import SparseFeatureHierarchy
 
-# where the transposed (finer-level) Gram entries go: "sorted" = atomic cursor + per-row segment sort,
-# "structural" = straight to the final slot from prefix tables (SPEC S6b).  solver_config['placement'] or the
-# NKSR_PLACEMENT environment variable override it.
-DEFAULT_PLACEMENT = "structural"
 # the layout every parity test runs on unless a test selects the other
 DEFAULT_ROW_LAYOUT = "levels"
 # the Gram fill (solver_config['fill'] or the NKSR_FILL environment variable override it): "brick", "rows", "grouped"
@@ -299,33 +295,25 @@ class KernelField(BaseField):
         dev = svh.device
         st = stream_ptr(dev)
         cnt = torch.empty(n, dtype=torch.int32, device=dev)
-        placement = self.solver_config.get("placement") or os.environ.get("NKSR_PLACEMENT") or DEFAULT_PLACEMENT
-        if placement not in ("sorted", "structural"):
-            raise ValueError("solver_config['placement'] must be 'sorted' or 'structural'")
-        place = None
-        if placement == "structural":
-            # transposed entries go straight to their final slot (SPEC S6b): per (fine level, offset) pair
-            # a rank table on the fine level and a 125-ancestor prefix table on the coarse level
-            cnt_down = torch.zeros(n, dtype=torch.int32, device=dev)
-            # row lengths with one column table per sibling group (fewer lookups than a walk per slot and row)
-            count = self.solver_config.get("count") or os.environ.get("NKSR_COUNT") or "grouped"
-            grouped = count == "grouped" and svh.depth <= 4 and svh.depth < _lib.MAX_DEPTH
-            call("nksr_gram_count_grouped" if grouped else "nksr_gram_count_own", svh.view(), cnt, st)
-            place = _lib.PlacementT()
-            for l in range(svh.depth - 1):
-                for k in range(1, svh.depth - l):
-                    n_lo, n_up = svh.num_voxels(l), svh.num_voxels(l + k)
-                    if n_lo == 0 or n_up == 0:
-                        continue
-                    rank8 = torch.empty((n_lo, 8), dtype=torch.int32, device=dev)
-                    classes = torch.empty((n_up, 27), dtype=torch.int32, device=dev)
-                    prefix = torch.empty((n_up, 125), dtype=torch.int32, device=dev)
-                    call("nksr_gram_place", svh.view(), l, k, rank8, classes, prefix, cnt_down, st)
-                    place.rank8[l][k], place.prefix[l][k] = rank8.data_ptr(), prefix.data_ptr()
-                    keep += [rank8, prefix]
-        else:
-            cnt_down = torch.empty(n, dtype=torch.int32, device=dev)
-            call("nksr_gram_count", svh.view(), cnt, cnt_down, st)
+        # transposed entries go straight to their final slot (SPEC S6b): per (fine level, offset) pair
+        # a rank table on the fine level and a 125-ancestor prefix table on the coarse level
+        cnt_down = torch.zeros(n, dtype=torch.int32, device=dev)
+        # row lengths with one column table per sibling group (fewer lookups than a walk per slot and row)
+        count = self.solver_config.get("count") or os.environ.get("NKSR_COUNT") or "grouped"
+        grouped = count == "grouped" and svh.depth <= 4 and svh.depth < _lib.MAX_DEPTH
+        call("nksr_gram_count_grouped" if grouped else "nksr_gram_count_own", svh.view(), cnt, st)
+        place = _lib.PlacementT()
+        for l in range(svh.depth - 1):
+            for k in range(1, svh.depth - l):
+                n_lo, n_up = svh.num_voxels(l), svh.num_voxels(l + k)
+                if n_lo == 0 or n_up == 0:
+                    continue
+                rank8 = torch.empty((n_lo, 8), dtype=torch.int32, device=dev)
+                classes = torch.empty((n_up, 27), dtype=torch.int32, device=dev)
+                prefix = torch.empty((n_up, 125), dtype=torch.int32, device=dev)
+                call("nksr_gram_place", svh.view(), l, k, rank8, classes, prefix, cnt_down, st)
+                place.rank8[l][k], place.prefix[l][k] = rank8.data_ptr(), prefix.data_ptr()
+                keep += [rank8, prefix]
         # (one spare row pointer, and below 4 spare entries of col / val: the streamed SpMV moves 16-byte units)
         rowptr = torch.zeros(n + 2, dtype=torch.int64, device=dev)[:n + 1]
         nb = call("nksr_scan_workspace_bytes", n)
@@ -452,30 +440,15 @@ class KernelField(BaseField):
         fill = self.solver_config.get("fill") or os.environ.get("NKSR_FILL") or DEFAULT_FILL
         if fill not in ("brick", "grouped", "rows"):
             raise ValueError("solver_config['fill'] must be 'brick', 'grouped' or 'rows'")
-        if place is not None and fill == "grouped" and svh.depth <= 4 and svh.depth < _lib.MAX_DEPTH:
+        if fill == "grouped" and svh.depth <= 4 and svh.depth < _lib.MAX_DEPTH:
             call("nksr_gram_fill_grouped", svh.view(), self.feat_view(), cs, cnt, rowptr, place, col, val, rhs, diag, st)
-        elif place is not None and fill == "brick":
+        elif fill == "brick":
             call("nksr_gram_fill_brick", svh.view(), self.feat_view(), cs, cnt, rowptr, place, col, val, rhs, diag,
                  float(BRICK_MIN_LOCATIONS_PER_VOXEL), st)
-        elif place is not None:
-            call("nksr_gram_fill_placed", svh.view(), self.feat_view(), cs, cnt, rowptr, place, col, val, rhs, diag, st)
         else:
-            cursor = torch.zeros(n, dtype=torch.int32, device=dev)
-            call("nksr_gram_fill", svh.view(), self.feat_view(), cs, cnt, rowptr, col, val, rhs, diag, cursor, st)
+            call("nksr_gram_fill_placed", svh.view(), self.feat_view(), cs, cnt, rowptr, place, col, val, rhs, diag, st)
         tm.mark("gram_fill")
-        # atomic-cursor variant: deterministic storage order of the transposed (finer-level) segments
-        # (rows binned by segment length so that short rows do not pay for a large tile)
-        offs = svh.offsets
-        if place is None and svh.depth > 1 and n > offs[1]:
-            seg = cnt_down[offs[1]:]
-            lo_b = 1
-            for cap in (32, 128, 512, 1024, 2048, 4096, 8192, 16384):
-                rows = (torch.nonzero((seg > lo_b) & (seg <= cap)).reshape(-1) + offs[1]).to(torch.int32)
-                lo_b = cap
-                if rows.numel():
-                    call("nksr_gram_sort_down", cnt, cnt_down, rowptr, rows, rows.numel(), cap, col, val, st)
         del keep
-        tm.mark("gram_sort")
         return SimpleNamespace(rowptr=rowptr, col=col, val=val, rhs=rhs, diag=diag, cnt=cnt, cnt_down=cnt_down,
                                n=n, nnz=nnz, cons=cons)
 

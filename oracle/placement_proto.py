@@ -1,5 +1,5 @@
-"""Prototype (numpy, TEST INFRASTRUCTURE ONLY) of the sort-free placement of the transposed
-cross-level Gram entries planned for round 2 (DESIGN.md section 7).
+"""Host reference (numpy, TEST INFRASTRUCTURE ONLY) for the sort-free placement of the transposed
+cross-level Gram entries (DESIGN.md SPEC S6b).
 
 Setting: fine voxel j (level l, offset-space coords u) stores an entry for coarse voxel c (level l+k) iff
 c lies in box_k(j) = [((u-1)>>k) - 1, ((u+1)>>k) + 1] per axis (SPEC S6).  With a = u >> k the ancestor of j,
@@ -12,8 +12,10 @@ in Morton order.  Ordering c's transposed segment by (slot of d, Morton index of
 
     position(j -> c) = prefix[c][slot(d)] + rank of j among the class(d) descendants of a
 
-and both tables come from linear prefix sums -- no atomics, no sort.  tests/test_cpu_placement.py checks
-the formula against a brute-force sort on real hierarchies."""
+and both tables come from linear prefix sums -- no atomics, no sort.  Finer levels come first (ascending), so the
+whole segment of c is ordered by (level, slot of d, Morton index); transposed_order gives that order for a whole
+hierarchy, and the GPU assembly is checked against it.  tests/test_cpu_placement.py checks the formula and
+transposed_order against a brute-force sort on real hierarchies."""
 from __future__ import annotations
 
 import numpy as np
@@ -21,6 +23,7 @@ import numpy as np
 from . import nksr_oracle as O
 
 _D5 = np.array([[a, b, c] for a in range(-2, 3) for b in range(-2, 3) for c in range(-2, 3)], np.int64)
+_OFF4 = np.array([[a, b, c] for a in range(4) for b in range(4) for c in range(4)], np.int64)
 
 
 def _edge_class(d):
@@ -100,3 +103,28 @@ def placement_by_sort(svh: O.OracleSVH, l: int, k: int):
         for pos, (_, j) in enumerate(sorted(lst)):
             out[(c, j)] = pos
     return out
+
+
+def transposed_order(svh: O.OracleSVH):
+    """-> (row, col): every transposed entry of the hierarchy (global unknown indices, levels concatenated), in the
+    storage order of SPEC S6b -- by row, then finer level (ascending), then slot of d = c - a, then Morton index."""
+    offs = svh.offsets()
+    rows, cols, lev, slot = [], [], [], []
+    for l in range(svh.depth):
+        fine = svh.ijk(l).astype(np.int64)
+        for lu in range(l + 1, svh.depth):
+            k = lu - l
+            cand = (((fine - 1) >> k) - 1)[:, None, :] + _OFF4[None]                 # the 4^3 box of every fine voxel
+            c = svh.lookup(lu, cand)
+            m = (c >= 0) & np.all(cand <= (((fine + 1) >> k) + 1)[:, None, :], axis=-1)
+            d = cand - (fine >> k)[:, None, :]
+            j = np.broadcast_to(np.arange(fine.shape[0])[:, None], m.shape)
+            rows.append(c[m] + offs[lu])
+            cols.append(j[m] + offs[l])
+            lev.append(np.full(int(m.sum()), l))
+            slot.append(((d + 2) * np.array([25, 5, 1])).sum(axis=-1)[m])
+    if not rows:
+        return np.zeros(0, np.int64), np.zeros(0, np.int64)
+    rows, cols, lev, slot = (np.concatenate(a) for a in (rows, cols, lev, slot))
+    order = np.lexsort((cols, slot, lev, rows))
+    return rows[order], cols[order]

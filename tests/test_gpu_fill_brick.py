@@ -53,7 +53,7 @@ def _hierarchy(cuda, xyz, W, L, prune=0.0, seed=0):
     return svh, osvh
 
 
-def _systems(cuda, svh, osvh, xyz, W, approx, split, normals, layout, placement, compact=False,
+def _systems(cuda, svh, osvh, xyz, W, approx, split, normals, layout, compact=False,
              fills=("rows", "brick", "brick")):
     import nksr_b200
     L = osvh.depth
@@ -67,8 +67,7 @@ def _systems(cuda, svh, osvh, xyz, W, approx, split, normals, layout, placement,
     out = []
     for fill in fills:
         field = nksr_b200.KernelField(svh, None, [t(f) for f in feats], approx)
-        field.solver_config.update(keep_system=True, max_iter=0, fill=fill, row_layout=layout, placement=placement,
-                                   compact_rows=compact)
+        field.solver_config.update(keep_system=True, max_iter=0, fill=fill, row_layout=layout, compact_rows=compact)
         if split is not None:
             field.solver_config["block_split_level"] = split
         if normals:
@@ -104,27 +103,31 @@ def _compare(out, ref, osvh, what):
     return worst
 
 
-@pytest.mark.parametrize("L,W,prune,approx,split,normals,layout,placement,compact", [
-    (4, 0.02, 0.0, False, None, True, "levels", "structural", False),      # bench settings: automatic split level
-    (4, 0.02, 0.0, True, None, True, "interleaved", "structural", False),
-    (4, 0.02, 0.5, True, 4, True, "levels", "structural", False),          # pruned finest level, every level bricked
-    (4, 0.02, 0.0, False, 4, True, "interleaved", "structural", False),
-    (4, 0.02, 0.0, False, 1, True, "levels", "structural", False),         # blocks from level 1: level 0 bricked
-    (4, 0.02, 0.0, False, 0, True, "interleaved", "structural", False),    # blocks everywhere: no brick
-    (4, 0.02, 0.0, False, None, True, "levels", "sorted", False),          # atomic-cursor placement: the row fill
-    (4, 0.02, 0.0, True, None, True, "levels", "structural", True),        # compact gradient rows: the row fill
-    (3, 0.03, 0.0, True, None, True, "interleaved", "structural", False),
-    (2, 0.04, 0.0, False, None, True, "levels", "structural", False),
-    (1, 0.05, 0.0, False, None, True, "interleaved", "structural", False),  # single level
-    (4, 0.02, 0.0, False, None, False, "levels", "structural", False),     # position constraints only
-    (5, 0.02, 0.0, False, None, True, "levels", "structural", False),      # depth > 4: the row fill
-])
-def test_brick_fill_is_the_row_fill(cuda, every_level, L, W, prune, approx, split, normals, layout, placement, compact):
+_CASES = [
+    (4, 0.02, 0.0, False, None, True, "levels", False),      # bench settings: automatic split level
+    (4, 0.02, 0.0, True, None, True, "interleaved", False),
+    (4, 0.02, 0.5, True, 4, True, "levels", False),          # pruned finest level, every level bricked
+    (4, 0.02, 0.0, False, 4, True, "interleaved", False),
+    (4, 0.02, 0.0, False, 1, True, "levels", False),         # blocks from level 1: level 0 bricked
+    (4, 0.02, 0.0, False, 0, True, "interleaved", False),    # blocks everywhere: no brick
+    (4, 0.02, 0.0, True, None, True, "levels", True),        # compact gradient rows: the row fill
+    (3, 0.03, 0.0, True, None, True, "interleaved", False),
+    (2, 0.04, 0.0, False, None, True, "levels", False),
+    (1, 0.05, 0.0, False, None, True, "interleaved", False),  # single level
+    (4, 0.02, 0.0, False, None, False, "levels", False),     # position constraints only
+    (5, 0.02, 0.0, False, None, True, "levels", False),      # depth > 4: the row fill
+]
+
+
+# (the ids keep the "structural" they had while the placement was a parameter, so every case keeps its history)
+@pytest.mark.parametrize("L,W,prune,approx,split,normals,layout,compact", _CASES,
+                         ids=["-".join(map(str, (*case[:-1], "structural", case[-1]))) for case in _CASES])
+def test_brick_fill_is_the_row_fill(cuda, every_level, L, W, prune, approx, split, normals, layout, compact):
     xyz, _ = clouds.shapenet_like(3000)
     svh, osvh = _hierarchy(cuda, xyz, W, L, prune)
-    out, ref = _systems(cuda, svh, osvh, xyz, W, approx, split, normals, layout, placement, compact)
+    out, ref = _systems(cuda, svh, osvh, xyz, W, approx, split, normals, layout, compact)
     worst = _compare(out, ref, osvh, f"L={L} W={W} prune={prune} approx={approx} split={split} normals={normals} "
-                                     f"{layout} {placement} compact={compact}")
+                                     f"{layout} compact={compact}")
     print(f"[brick] worst reorder ratios (values, diagonal, rhs): {worst}")
 
 
@@ -132,8 +135,8 @@ def test_brick_layouts_give_the_same_system(cuda, every_level):
     """the brick fill under both row layouts: same products in the same order, bitwise the same system"""
     xyz, _ = clouds.shapenet_like(3000)
     svh, osvh = _hierarchy(cuda, xyz, 0.02, 4)
-    (a,), _ = _systems(cuda, svh, osvh, xyz, 0.02, False, 4, True, "levels", "structural", fills=("brick",))
-    (b,), _ = _systems(cuda, svh, osvh, xyz, 0.02, False, 4, True, "interleaved", "structural", fills=("brick",))
+    (a,), _ = _systems(cuda, svh, osvh, xyz, 0.02, False, 4, True, "levels", fills=("brick",))
+    (b,), _ = _systems(cuda, svh, osvh, xyz, 0.02, False, 4, True, "interleaved", fills=("brick",))
     for name in ("rowptr", "col", "val", "rhs", "diag"):
         assert torch.equal(getattr(a, name), getattr(b, name)), name
 
@@ -152,7 +155,7 @@ def test_brick_edge_cases(cuda, every_level):
         svh, osvh = _hierarchy(cuda, xyz, W, L, prune, seed=L)
         if L == 4:
             assert osvh.n(L - 1) <= 64
-        out, ref = _systems(cuda, svh, osvh, xyz, W, False, split, True, "levels", "structural")
+        out, ref = _systems(cuda, svh, osvh, xyz, W, False, split, True, "levels")
         _compare(out, ref, osvh, f"edge L={L} prune={prune} split={split}")
 
 
@@ -163,8 +166,7 @@ def test_sparse_levels_take_the_row_fill(cuda, monkeypatch):
     monkeypatch.setattr(fields, "BRICK_MIN_LOCATIONS_PER_VOXEL", 1e9)
     xyz, _ = clouds.shapenet_like(3000)
     svh, osvh = _hierarchy(cuda, xyz, 0.02, 4)
-    (rows, brick), _ = _systems(cuda, svh, osvh, xyz, 0.02, False, 4, True, "levels", "structural",
-                                fills=("rows", "brick"))
+    (rows, brick), _ = _systems(cuda, svh, osvh, xyz, 0.02, False, 4, True, "levels", fills=("rows", "brick"))
     for name in ("rowptr", "col", "val", "rhs", "diag"):
         assert torch.equal(getattr(rows, name), getattr(brick, name)), name
 

@@ -116,18 +116,22 @@ def test_interleaved_rows_are_the_level_rows(cuda, L, C, approx):
         assert float(plain.abs().max()) > 0
 
 
-@pytest.mark.parametrize("L,W,approx,split,normals,placement", [
-    (4, 0.02, False, None, True, "structural"),   # automatic split level: blocks on the two coarse levels
-    (4, 0.02, True, None, True, "structural"),
-    (4, 0.02, False, 4, True, "structural"),      # every level through the row loops
-    (4, 0.02, False, 1, True, "structural"),      # blocks from level 1
-    (4, 0.02, False, 0, True, "structural"),      # blocks everywhere
-    (4, 0.02, False, None, True, "sorted"),       # atomic-cursor placement + segment sort
-    (3, 0.03, False, None, True, "structural"),   # a level the layout pads with zeros
-    (1, 0.05, False, None, True, "structural"),
-    (4, 0.02, False, None, False, "structural"),  # position constraints only
-])
-def test_interleaved_layout_gives_the_same_system(cuda, L, W, approx, split, normals, placement):
+_LAYOUT_CASES = [
+    (4, 0.02, False, None, True),     # automatic split level: blocks on the two coarse levels
+    (4, 0.02, True, None, True),
+    (4, 0.02, False, 4, True),        # every level through the row loops
+    (4, 0.02, False, 1, True),        # blocks from level 1
+    (4, 0.02, False, 0, True),        # blocks everywhere
+    (3, 0.03, False, None, True),     # a level the layout pads with zeros
+    (1, 0.05, False, None, True),
+    (4, 0.02, False, None, False),    # position constraints only
+]
+
+
+# (the ids keep the "structural" they had while the placement was a parameter, so every case keeps its history)
+@pytest.mark.parametrize("L,W,approx,split,normals", _LAYOUT_CASES,
+                         ids=["-".join(map(str, case)) + "-structural" for case in _LAYOUT_CASES])
+def test_interleaved_layout_gives_the_same_system(cuda, L, W, approx, split, normals):
     """solver_config['row_layout'] = 'interleaved' (csrc/assemble.cu, ILV: 128-bit loads of all levels of a location)
     against 'levels': same products in the same order -- row pointers, columns, values, rhs and diagonal are bitwise
     equal, through the row loops and through the per-voxel blocks."""
@@ -144,7 +148,7 @@ def test_interleaved_layout_gives_the_same_system(cuda, L, W, approx, split, nor
     out = []
     for layout in ("levels", "interleaved"):
         field = _field(cuda, svh, feats, approx)
-        field.solver_config.update(keep_system=True, max_iter=0, row_layout=layout, placement=placement)
+        field.solver_config.update(keep_system=True, max_iter=0, row_layout=layout)
         if split is not None:
             field.solver_config["block_split_level"] = split
         if normals:
@@ -248,11 +252,15 @@ def test_gram_assembly_matches_oracle(cuda, C, approx, compact, split):
 
 
 @pytest.mark.parametrize("L,W,prune", [(4, 0.02, False), (2, 0.04, False), (5, 0.02, False), (3, 0.03, True)])
-def test_structural_placement_is_the_same_matrix(cuda, L, W, prune):
-    """SPEC S6b: placing the transposed entries from prefix tables (no atomics, no sort) stores exactly the
-    matrix of the atomic-cursor + sort variant -- same pattern, bitwise the same values, same row lengths --
-    and is itself run-to-run identical in storage order."""
+def test_structural_placement_is_the_same_matrix(cuda, monkeypatch, L, W, prune):
+    """SPEC S6b, with the row fill and with the default brick fill (every level below the split bricked): the transposed
+    entries, placed from prefix tables (no atomics, no sort), give row lengths that split the structural pattern at the
+    level offsets, fill every slot once, stand in every row's finer-level segment in the order of the host reference
+    (placement_proto.transposed_order), each hold bitwise the entry they copy, and are stored identically run to run."""
     import nksr_b200
+    from nksr_b200 import fields
+    from oracle import placement_proto as PP
+    monkeypatch.setattr(fields, "BRICK_MIN_LOCATIONS_PER_VOXEL", 0.0)
     xyz, _ = clouds.shapenet_like(3000)
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(cuda)
     osvh = O.OracleSVH(W, L).build_point_splatting(xyz)
@@ -265,21 +273,44 @@ def test_structural_placement_is_the_same_matrix(cuda, L, W, prune):
     nxyz = np.concatenate([osvh.centers(d) for d in range(min(2, L))])
     nval = -(nxyz / np.linalg.norm(nxyz, axis=1, keepdims=True)).astype(np.float32)
     pw, nw = 1e4 / xyz.shape[0], 1e4 / nxyz.shape[0] * W * W
-    out = {}
-    for placement in ("sorted", "structural", "structural"):
-        field = _field(cuda, svh, feats, False)
-        field.solver_config.update(keep_system=True, max_iter=0, placement=placement, fill="rows")
-        field.solve(t(xyz), t(nxyz), t(nval), pw, nw, 1.0)
-        s = field.system
-        out.setdefault(placement, []).append((_np(s.rowptr).copy(), _np(s.col).copy(), _np(s.val).copy(), _gpu_csr(field)))
-    (rp_s, _, _, A_s), (rp_a, col_a, val_a, A_a), (rp_b, col_b, val_b, _) = out["sorted"][0], *out["structural"]
-    assert np.array_equal(rp_s, rp_a) and A_s.nnz == A_a.nnz
-    A_s.sum_duplicates(); A_a.sum_duplicates()
-    assert A_a.nnz == rp_a[-1] and (A_s != A_a).nnz == 0                # no duplicate slot, identical entries
-    assert np.array_equal(rp_a, rp_b) and np.array_equal(col_a, col_b) and np.array_equal(val_a, val_b)
-    P = O.structural_pattern(osvh)
-    Ab = A_a.copy(); Ab.data[:] = 1
-    assert Ab.nnz == P.nnz and (Ab - P).count_nonzero() == 0
+    pattern = O.structural_pattern(osvh)
+    P = pattern.tocoo()
+    offs = osvh.offsets()
+    n = int(offs[-1])
+    level = lambda i: np.searchsorted(offs, i, side="right") - 1
+    finer = level(P.col) < level(P.row)
+    cnt_ref = np.bincount(P.row[~finer], minlength=n)
+    down_ref = np.bincount(P.row[finer], minlength=n)
+    order_rows, order_cols = PP.transposed_order(osvh)
+    assert order_cols.shape[0] == int(down_ref.sum()) > 0
+    for fill in ("rows", "brick"):
+        out = []
+        for _ in range(2):
+            field = _field(cuda, svh, feats, False)
+            field.solver_config.update(keep_system=True, max_iter=0, fill=fill)
+            field.solve(t(xyz), t(nxyz), t(nval), pw, nw, 1.0)
+            s = field.system
+            out.append([_np(a).copy() for a in (s.rowptr, s.col, s.val, s.cnt, s.cnt_down)])
+        (rp, col, val, cnt, cnt_down), again = out
+        # row lengths and pattern: no slot written twice, none left unwritten
+        assert np.array_equal(cnt, cnt_ref) and np.array_equal(cnt_down, down_ref), fill
+        assert np.array_equal(rp, np.concatenate([[0], np.cumsum(cnt_ref + down_ref)])), fill
+        A = sp.csr_matrix((np.ones(col.shape[0]), col, rp), shape=(n, n), copy=True)   # (sum_duplicates sorts in place)
+        A.sum_duplicates()
+        assert A.nnz == rp[-1] and (A - pattern).count_nonzero() == 0, fill
+        # the finer-level segment of every row in the S6b order
+        row_of = np.repeat(np.arange(n), np.diff(rp))
+        down = np.arange(rp[-1]) - rp[row_of] >= cnt[row_of]
+        assert np.array_equal(row_of[down], order_rows) and np.array_equal(col[down], order_cols), fill
+        # every transposed copy (c, j) is bitwise the value row j stores for column c
+        own_key = row_of[~down] * n + col[~down]
+        srt = np.argsort(own_key)
+        src_key = col[down].astype(np.int64) * n + row_of[down]
+        at = np.minimum(np.searchsorted(own_key[srt], src_key), own_key.size - 1)
+        assert np.array_equal(own_key[srt][at], src_key), fill
+        assert np.array_equal(val[~down][srt][at].view(np.uint32), val[down].view(np.uint32)), fill
+        for a, b in zip(out[0][:3], again[:3]):
+            assert np.array_equal(a, b), fill
 
 
 @pytest.mark.parametrize("L,W,prune,approx,compact,split,normals", [

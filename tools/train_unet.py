@@ -144,7 +144,7 @@ def main(argv=None):
             st = stages.report()
             kern = {name: round(float(v), 6) for name, v in out[2].items()}
             kern.update(kernel_solve_ms=round(sum(st.get(s, 0.0) for s in ("kernel_rows", "gram_count", "gram_blocks",
-                                                                           "gram_fill", "gram_sort", "pcg")), 3),
+                                                                           "gram_fill", "pcg")), 3),
                         adjoint_pcg_ms=round(st.get("adjoint_pcg", 0.0), 3),
                         vjp_ms=round(st.get("feature_vjp", 0.0) + st.get("evaluate_vjp", 0.0), 3))
         row = dict(step=step, structure=round(float(l_struct), 6), udf=round(float(l_udf), 6), **kern,
