@@ -124,6 +124,22 @@ NKSR_API int nksr_gather_gemm_wgrad(const float* x, const int32_t* idx, int64_t 
  * zeroed by the caller) |= 1 when two rows share a (source, tap), |= 2 when a source is >= n_src. */
 NKSR_API int nksr_transpose_taps(const int32_t* idx, int64_t n_out, int K, int64_t n_src, int32_t* idx_t,
                         int32_t* status, void* stream);
+/* ---- f2b: the structure-grown decoder hierarchy (DESIGN.md SPEC S16; models/nksr_net.py:74-86, dec_tmp_svh).
+ * classify: per voxel of level `level`, c = argmax of the 3 logits at logits[i*row_stride] (torch.argmax semantics:
+ * first index on a tie, NaN largest), or c = forced[i] when forced != NULL; cls[i] = c, keep[i] = c >= 1,
+ * sub[i] = level >= 1 && (c == 2 || (c == 1 && level >= adaptive_depth)). */
+NKSR_API int nksr_structure_classify(const float* logits, int64_t row_stride, const int32_t* forced, int64_t n,
+                                     int level, int adaptive_depth, int8_t* cls, int32_t* keep, int32_t* sub,
+                                     void* stream);
+/* children of the subdivided voxels of one level (sub_scan = nksr_exclusive_scan32 of sub, n + 1 entries; the caller
+ * sizes the child arrays 8 * sub_scan[n]): child c = 8 sub_scan[i] + o of voxel i has key (keys[i] << 3) | o, parent i
+ * and join enc_child8[join[i]*8 + o] (-1 when join[i] < 0 or enc_child8 == NULL); child8 (n x 8) = c, or -1 rows for
+ * voxels that are not subdivided.  Deterministic: no atomics, no sort. */
+NKSR_API int nksr_structure_grow(const int64_t* keys, const int32_t* sub, const int64_t* sub_scan, int64_t n,
+                                 const int32_t* join, const int32_t* enc_child8, int64_t* child_keys,
+                                 int32_t* child_parent, int32_t* child_join, int32_t* child8, void* stream);
+/* table composition out[i*K+k] = idx[i*K+k] < 0 ? -1 : map[idx[i*K+k]] (n rows of K taps) */
+NKSR_API int nksr_compose_taps(const int32_t* idx, int64_t n, int K, const int32_t* map, int32_t* out, void* stream);
 /* first/last+1 sorted location of every level-l voxel: range[2*u], range[2*u+1] */
 NKSR_API int nksr_row_ranges(const int32_t* base_l, int64_t m, int32_t* range, int64_t n_l, void* stream);
 

@@ -69,6 +69,9 @@ _SIGNATURES = {
     "nksr_gather_gemm_wgrad_workspace_bytes": ("z", "qiiii"),
     "nksr_gather_gemm_wgrad": ("i", "ppqipiipppzip"),
     "nksr_transpose_taps": ("i", "pqiqppp"),
+    "nksr_structure_classify": ("i", "pqpqiippp" + "p"),
+    "nksr_structure_grow": ("i", "pppqppppppp"),
+    "nksr_compose_taps": ("i", "pqippp"),
     "nksr_build_rows": ("i", "SFppqiipp"),
     "nksr_build_rows_voxel": ("i", "SFpppqiipp"),
     "nksr_scan_workspace_bytes": ("z", "q"),

@@ -288,6 +288,10 @@ def reconstruct_global(reconstructor, xyz: torch.Tensor, normal: Optional[torch.
     (each keeps its slab + halo); True: every rank passes ITS SHARE of the cloud and the points are routed to
     the ranks that need them by one all-to-all.  Returns a KernelField over this rank's slab+halo region with
     `.owned` (per-unknown bool), `.owned_cells` (level-0 mask for meshing) and `.solve_info`."""
+    if getattr(reconstructor.network, "structure", "encoder") == "predicted":
+        # every rank would grow its own hierarchy from its own predictions, which can disagree in the halo
+        raise _lib.NksrError("the global solve needs structure='encoder': hierarchies grown from the predicted "
+                             "structure are not kept consistent across ranks")
     world, rank = _world(group), _rank(group)
     dev = reconstructor.device
     xyz = xyz.detach().to(dev, torch.float32).contiguous()

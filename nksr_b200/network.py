@@ -12,7 +12,12 @@ seeded, deterministic replacement that produces the SAME OUTPUT CONTRACT the hot
     feat.structure_features[d] (n_d, 3)         feat.udf_features[d]
     network.interpolators / .sdf_decoder / .udf_decoder
 
-Normals are the pooled input normals (or view directions) -- i.e. the "prediction" is
+With backbone='unet', `structure` chooses the decoder hierarchy: 'encoder' (default) decodes on the encoder hierarchy and
+returns it as dec_svh and udf_svh; 'predicted' grows it from the structure head level by level (DESIGN.md SPEC S16,
+nksr_b200/structure.py) -- teacher-forced from gt_decoder_svh when one is given -- and returns the kept voxels as dec_svh
+and the whole grown hierarchy (the reference's dec_tmp_svh) as udf_svh.
+
+For backbone='pool', normals are the pooled input normals (or view directions) -- i.e. the "prediction" is
 geometric, not learned; kernel features are a seeded perturbation of a constant, which makes
 the kernel close to the pure Bezier kernel (well conditioned).  Documented as synthetic in
 bench.py (`"data": "synthetic"`).
@@ -28,7 +33,8 @@ from .svh import SparseFeatureHierarchy
 
 _DEFAULTS = dict(kernel_dim=4, tree_depth=4, adaptive_depth=2, feature="normal",
                  interpolator=dict(n_hidden=2, hidden_dim=16), udf=dict(enabled=False), seed=0,
-                 unet=dict(f_maps=32), backbone="pool", precision="fp32", trainable=False)
+                 unet=dict(f_maps=32), backbone="pool", precision="fp32", trainable=False, structure="encoder",
+                 structure_max_ratio=None)
 
 
 def _get(hp, key, default):
@@ -80,6 +86,17 @@ class NKSRNetwork(nn.Module):
         self.trainable = bool(hp["trainable"])
         if self.trainable and self.backbone != "unet":
             raise ValueError("trainable=True needs backbone='unet' (the 'pool' stand-in has nothing to train)")
+        # structure: 'encoder' = the decoder runs on the encoder hierarchy; 'predicted' = it grows its own hierarchy
+        # from the structure head, level by level (DESIGN.md SPEC S16, nksr_b200/structure.py) -- U-Net backbone only
+        self.structure = str(hp["structure"])
+        if self.structure not in ("encoder", "predicted"):
+            raise ValueError("structure: 'encoder' or 'predicted'")
+        if self.structure == "predicted" and self.backbone != "unet":
+            raise ValueError("structure='predicted' needs backbone='unet' (the 'pool' stand-in has no structure head "
+                             "to grow from)")
+        # children a grown level may hold, as a multiple of the encoder voxels of that level (None: the default of
+        # nksr_b200/structure.py, DEFAULT_MAX_RATIO)
+        self.structure_max_ratio = hp["structure_max_ratio"]
         interp = hp["interpolator"]
         gen = torch.Generator().manual_seed(int(hp["seed"]))
         state = torch.random.get_rng_state()
@@ -148,12 +165,14 @@ class NKSRNetwork(nn.Module):
             return self._unet(feat, svh, adaptive_depth, gt_decoder_svh)
 
     def _unet(self, feat, svh, adaptive_depth, gt_decoder_svh):
+        if self.structure == "predicted":
+            return self._unet_grown(feat, svh, adaptive_depth, gt_decoder_svh)
         dec_svh = gt_decoder_svh if gt_decoder_svh is not None else svh
         C = self.kernel_dim
         if self.backbone == "unet":
-            # the decoder runs on the encoder hierarchy; a given decoder hierarchy (ground truth at training time,
-            # models/nksr_net.py:77) receives the features of the voxels it shares with it.  Growing the decoder
-            # hierarchy from the predicted structure logits needs trained weights and is not done here.
+            # structure='encoder': the decoder runs on the encoder hierarchy; a given decoder hierarchy (ground truth at
+            # training time, models/nksr_net.py:77) receives the features of the voxels it shares with it.
+            # structure='predicted' grows the decoder hierarchy from the structure logits instead (_unet_grown).
             from .unet import restrict_to
             o = self.backbone_net(feat.x0, svh, tf32=self.tf32)
             return (FeatureBundle(basis_features=restrict_to(o.basis, svh, dec_svh),
@@ -179,6 +198,22 @@ class NKSRNetwork(nn.Module):
         out = FeatureBundle(basis_features=basis, normal_features=normal, structure_features=structure,
                             udf_features=udf)
         return out, dec_svh, dec_svh
+
+    def _unet_grown(self, feat, svh, adaptive_depth, gt_decoder_svh, impl="cuda"):
+        """structure='predicted' (DESIGN.md SPEC S16): the decoder grows its hierarchy T from its structure logits, or
+        from gt_decoder_svh's voxel status when one is given (teacher forcing, models/nksr_net.py:74-86).  Returns
+        (features, dec_svh, udf_svh): udf_svh = T, where the structure and UDF features live; dec_svh = T's kept voxels,
+        where the basis and normal features live."""
+        from .structure import teacher_classes
+        ad = self.adaptive_depth if adaptive_depth is None else int(adaptive_depth)
+        forced = teacher_classes(gt_decoder_svh) if gt_decoder_svh is not None else None
+        o = self.backbone_net(feat.x0, svh, tf32=self.tf32, impl=impl,
+                              grow=dict(adaptive_depth=ad, forced=forced, max_ratio=self.structure_max_ratio))
+        kept = o.kept
+        bundle = FeatureBundle(basis_features={l: f[kept[l]] for l, f in o.basis.items()},
+                               normal_features={l: f[kept[l]] for l, f in o.normal.items()},
+                               structure_features=o.structure, udf_features=o.udf, classes=o.classes)
+        return bundle, o.dec_svh, o.udf_svh
 
 
 def load_checkpoint_from_url(url: str):

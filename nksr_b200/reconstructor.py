@@ -338,6 +338,8 @@ class Reconstructor:
         tm.mark("svh_build")
         enc = self.network.encoder(xyz, feat, svh, 0)
         feats, dec_svh, _ = self.network.unet(enc, svh, adaptive_depth=self.adaptive_depth)
+        if getattr(self.network, "structure", "encoder") == "predicted" and dec_svh.num_unknowns == 0:
+            raise _lib.NksrError("predicted structure is empty: the network kept no voxel, there is nothing to solve")
         field = KernelField(dec_svh, self.network.interpolators, feats.basis_features, approx_kernel_grad)
         field._timer = tm
         tm.mark("network")
@@ -363,6 +365,11 @@ class Reconstructor:
         normal = normal.detach().to(self.device, torch.float32).contiguous() if normal is not None else None
         sensor = sensor.detach().to(self.device, torch.float32).contiguous() if sensor is not None else None
         if chunk_size is not None and chunk_size > 0:
+            if getattr(self.network, "structure", "encoder") == "predicted":
+                # the blended field is meshed on one union hierarchy built from the points (SPEC S14), which a grown
+                # per-chunk hierarchy would not match
+                raise _lib.NksrError("chunk mode needs structure='encoder': chunked reconstruction on hierarchies grown "
+                                     "from the predicted structure is not supported")
             # NKSR-USAGE.md:137: detail_level / voxel_size are not tunable in chunk mode
             voxel_size = DEFAULT_VOXEL_SIZE
             return self._reconstruct_chunks(xyz, normal, sensor, voxel_size, float(chunk_size), preprocess_fn,

@@ -112,6 +112,17 @@ class SparseFeatureHierarchy:
         self.adaptive_depth = min(int(adaptive_depth), self.depth)
         return out
 
+    def build_from_structure(self, enc_svh: "SparseFeatureHierarchy", classes_by_level, adaptive_depth: int):
+        """The decoder hierarchy grown from explicit structure classes over an encoder hierarchy (DESIGN.md SPEC S16):
+        classes_by_level[l] (0 empty, 1 leaf, 2 subdivide) for every voxel of level l of the grown hierarchy T, or a
+        function (T, l) -> those classes, for the levels 0 .. self.depth - 1 (T's coarsest level is enc_svh's).  This
+        hierarchy becomes the kept voxels of T; `adaptive_depth` says below which level a leaf stays a leaf."""
+        from .structure import grow_from_classes
+        if len(classes_by_level) != self.depth:
+            raise ValueError(f"{len(classes_by_level)} levels of classes for a depth-{self.depth} hierarchy")
+        grow_from_classes(enc_svh, classes_by_level, adaptive_depth, dec=self)
+        return self
+
     def build_from_keys(self, keys, top_keys=None):
         """Adopt sorted, unique, parent-closed Morton keys per level and build the tables.
         `top_keys`: keys of the virtual level above the coarsest one (default: its parents)."""

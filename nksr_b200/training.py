@@ -109,7 +109,10 @@ def udf_loss(udf_decoder, udf_features, svh: SparseFeatureHierarchy, ref_xyz, re
              samplers=UDF_SAMPLERS, gt_band=GT_BAND, generator=None, q=None):
     """mean |transform(pd) - gt| / voxel_size over the UDF samples (models/loss.py:120-140).  pd is the UDF NeuralField
     evaluated differentiably as udf_decoder(NeuralField._interp(q)) on the finest level's UDF features (the decoder
-    takes kernel_dim inputs); `q` overrides the samplers."""
+    takes kernel_dim inputs); `q` overrides the samplers.  Zero when the finest level is empty (a hierarchy grown from
+    a prediction that kept nothing there): there is no field to evaluate."""
+    if svh.num_voxels(0) == 0:
+        return torch.zeros((), device=svh.device)
     if q is None:
         q = udf_samples(svh, ref_xyz, ref_normal, voxel_size, samplers, generator)
     gt = udf_gt(q, ref_xyz, ref_normal, voxel_size, gt_band)
@@ -182,13 +185,35 @@ def kernel_losses(net, scene: TrainingScene, generator=None, feat=None, dec_svh=
     return dict(total=total, gt_value=l_val, gt_normal=l_nrm, spatial=l_sp, field=field)
 
 
-def losses(net, scene: TrainingScene, generator=None, kernel=False, timer=None):
+def use_predicted_structure(pd_structure_prob, generator=None):
+    """whether this step grows the decoder from the network's own structure prediction instead of teacher forcing
+    (the reference's should_use_pd_structure, models/nksr_net.py:218-226): never for a probability <= 0, always for
+    >= 1, else a draw from `generator` (only then is one consumed, so that the default keeps every random stream as
+    it was)"""
+    p = float(pd_structure_prob)
+    if p <= 0.0:
+        return False
+    if p >= 1.0:
+        return True
+    dev = generator.device if generator is not None else "cpu"
+    return bool(torch.rand((1,), generator=generator, device=dev).item() < p)
+
+
+def losses(net, scene: TrainingScene, generator=None, kernel=False, timer=None, pd_structure_prob=0.0):
     """forward of a trainable NKSRNetwork on the scene and its weighted losses: (total, structure, udf), and with
-    `kernel` the kernel_losses dict as a fourth element (its total is included in the first)"""
+    `kernel` the kernel_losses dict as a fourth element (its total is included in the first).  The structure and UDF
+    losses live on the third hierarchy unet() returns: the encoder hierarchy for structure='encoder', the grown one for
+    structure='predicted' -- teacher-forced from the scene's ground truth, or grown from the prediction with
+    probability `pd_structure_prob`."""
     enc = net.encoder(scene.xyz, scene.normal, scene.enc_svh, 0)
-    feat, dec_svh, _ = net.unet(enc, scene.enc_svh, adaptive_depth=scene.adaptive_depth)
-    l_struct, _ = structure_loss(feat.structure_features, dec_svh, scene.gt_svh)
-    l_udf = udf_loss(net.udf_decoder, feat.udf_features, dec_svh, scene.xyz, scene.normal, scene.voxel_size,
+    if getattr(net, "structure", "encoder") == "predicted":
+        gt_dec = None if use_predicted_structure(pd_structure_prob, generator) else scene.gt_svh
+        feat, dec_svh, udf_svh = net.unet(enc, scene.enc_svh, adaptive_depth=scene.adaptive_depth,
+                                          gt_decoder_svh=gt_dec)
+    else:
+        feat, dec_svh, udf_svh = net.unet(enc, scene.enc_svh, adaptive_depth=scene.adaptive_depth)
+    l_struct, _ = structure_loss(feat.structure_features, udf_svh, scene.gt_svh)
+    l_udf = udf_loss(net.udf_decoder, feat.udf_features, udf_svh, scene.xyz, scene.normal, scene.voxel_size,
                      generator=generator)
     total = STRUCTURE_WEIGHT * l_struct + UDF_WEIGHT * l_udf
     if not kernel:
@@ -205,13 +230,15 @@ def make_optimizer(net):
     return torch.optim.Adam([p for p in net.parameters() if p.requires_grad], lr=LEARNING_RATE)
 
 
-def train_step(net, opt, scene: TrainingScene, generator=None, marks=None, kernel=False, timer=None):
+def train_step(net, opt, scene: TrainingScene, generator=None, marks=None, kernel=False, timer=None,
+               pd_structure_prob=0.0):
     """one Adam step (gradient norm clipped to GRAD_CLIP); returns the (structure, udf) losses as tensors, and with
     `kernel` (the kernel-field losses added, trained through the kernel solve) a third element: the dict of the
     detached kernel losses.  `marks`, if given, is called with 'forward' / 'backward' / 'step' after each phase has
-    been enqueued; `timer` (a StageTimer) receives the kernel solve's stage marks."""
+    been enqueued; `timer` (a StageTimer) receives the kernel solve's stage marks.  `pd_structure_prob`: see
+    `losses` (structure='predicted' only)."""
     opt.zero_grad(set_to_none=True)
-    out = losses(net, scene, generator, kernel, timer)
+    out = losses(net, scene, generator, kernel, timer, pd_structure_prob)
     total, l_struct, l_udf = out[:3]
     if marks:
         marks("forward")

@@ -144,13 +144,24 @@ def transposed_table(svh, idx, n_src):
 _KERNEL_FLAG = {0: 0, 1: 2, 2: 2, 3: 3}          # the weights are always rounded on the host (flag 2), never per fragment
 
 
+def _per_part(idx, n_parts):
+    """one gather table per part: `idx` itself when it is a tuple / list of them, else the one table for every part"""
+    if isinstance(idx, (tuple, list)):
+        if len(idx) != n_parts:
+            raise ValueError(f"{len(idx)} index tables for {n_parts} parts")
+        return tuple(idx)
+    return (idx,) * n_parts
+
+
 def conv_parts(parts, idx, weights, bias, res, relu, mode):
     """y = act(bias + res + sum_p conv(parts[p], weights[p])): the convolution of the channel concatenation of `parts`
-    without materialising it -- one kernel call per part, each adding to the previous one's output"""
+    without materialising it -- one kernel call per part, each adding to the previous one's output.  `idx`: one table
+    for all parts, or one per part (the decoder's skip input comes from another hierarchy through its own table)."""
     y = res
+    idxs = _per_part(idx, len(parts))
     for i, (x, w) in enumerate(zip(parts, weights)):
         last = i == len(parts) - 1
-        y = gather_gemm(x, idx, w, bias if last else None, y, relu and last, _KERNEL_FLAG[int(mode)])
+        y = gather_gemm(x, idxs[i], w, bias if last else None, y, relu and last, _KERNEL_FLAG[int(mode)])
     return y
 
 
@@ -159,7 +170,9 @@ class GatherConv(torch.autograd.Function):
     itself (the same kernels and bits as without grad).  Backward, with g = dY * [y > 0] under ReLU (relu'(0) = 0):
       d_res = g,  d_bias = sum_i g[i],  dW = the weight-gradient kernel per part, concatenated along c_in,
       d_part_p = the forward kernel over the transposed table with part p's slice of W_k^T.
-    idx_t: the transposed table, a function returning it (called once, in backward), or None (computed in backward)."""
+    idx_t: the transposed table, a function returning it (called once, in backward), or None (computed in backward).
+    With one table per part (`idx` a tuple), every part's weight and input gradient run over its own table, and idx_t
+    is a tuple of one such entry per part (or None)."""
 
     @staticmethod
     def forward(ctx, idx, idx_t, mode, relu, weight, bias, res, *parts):
@@ -179,22 +192,30 @@ class GatherConv(torch.autograd.Function):
         d_w = d_b = d_res = None
         if need[6]:
             d_res = g
+        idxs = _per_part(ctx.idx, len(parts))
         if need[4] or need[5]:
             dws = []
             for p, x in enumerate(parts):
-                dw, db = gather_gemm_wgrad(x, ctx.idx, g, ctx.mode, bias=p == 0 and need[5])
+                dw, db = gather_gemm_wgrad(x, idxs[p], g, ctx.mode, bias=p == 0 and need[5])
                 dws.append(dw)
                 d_b = db if p == 0 else d_b
             d_w = dws[0] if len(dws) == 1 else torch.cat(dws, dim=1)
         d_parts = [None] * len(parts)
         if any(need[7:]):
-            idx_t = ctx.idx_t() if callable(ctx.idx_t) else ctx.idx_t
-            if idx_t is None:
-                idx_t = transpose_taps(ctx.idx, parts[0].shape[0])
+            if isinstance(ctx.idx, (tuple, list)):
+                idx_ts = ctx.idx_t if isinstance(ctx.idx_t, (tuple, list)) else (None,) * len(parts)
+            else:
+                idx_t = ctx.idx_t() if callable(ctx.idx_t) else ctx.idx_t
+                if idx_t is None:
+                    idx_t = transpose_taps(ctx.idx, parts[0].shape[0])
+                idx_ts = (idx_t,) * len(parts)
             wts = kernel_weights(weight, ctx.mode, ctx.splits, transposed=True)
             for p in range(len(parts)):
                 if need[7 + p]:
-                    d_parts[p] = gather_gemm(g, idx_t, wts[p], None, None, False, _KERNEL_FLAG[ctx.mode])
+                    t = idx_ts[p]() if callable(idx_ts[p]) else idx_ts[p]
+                    if t is None:
+                        t = transpose_taps(idxs[p], parts[p].shape[0])
+                    d_parts[p] = gather_gemm(g, t, wts[p], None, None, False, _KERNEL_FLAG[ctx.mode])
         return (None, None, None, None, d_w, d_b, d_res, *d_parts)
 
 
@@ -204,7 +225,8 @@ def _wants_grad(*tensors):
 
 class SparseConv(nn.Module):
     """K-tap sparse convolution: weight (K, c_in, c_out) + bias; the taps' sources come from an index table.  `x` may be
-    a tuple of tensors: the convolution then runs over their channel concatenation (the U-Net's skip connections).
+    a tuple of tensors: the convolution then runs over their channel concatenation (the U-Net's skip connections);
+    `idx` is then one table for all of them or a tuple of one table per part (and `idx_t` one entry per part).
     With grad enabled and an input or parameter that requires grad, the CUDA path runs through `GatherConv`; `idx_t`
     (the transposed table or a function returning it) saves its computation in backward."""
 
@@ -218,6 +240,14 @@ class SparseConv(nn.Module):
     def forward(self, x, idx, res=None, relu=True, tf32=False, impl="cuda", idx_t=None):
         parts = tuple(x) if isinstance(x, (tuple, list)) else (x,)
         if impl != "cuda":
+            if isinstance(idx, (tuple, list)):          # one table per part: the sum of the per-part convolutions
+                ws = torch.split(self.weight, [int(q.shape[1]) for q in parts], dim=1)
+                y = sum(gather_gemm(q, t, w, None, None, False, False, impl)
+                        for q, t, w in zip(parts, _per_part(idx, len(parts)), ws))
+                y = y + self.bias
+                if res is not None:
+                    y = y + res
+                return torch.relu(y) if relu else y
             xc = parts[0] if len(parts) == 1 else torch.cat(parts, dim=1)
             return gather_gemm(xc, idx, self.weight, self.bias, res, relu, False, impl)
         mode = int(tf32)
@@ -332,12 +362,9 @@ class SparseUNet(nn.Module):
                 out[rows] = y_coarse[parent[rows]] @ self.up[l][o]
         return out
 
-    def forward(self, x0, svh, tf32=False, impl="cuda"):
-        D = min(self.depth, svh.depth)
-        kw = dict(tf32=tf32, impl=impl)
+    def _encode(self, x0, svh, D, kw, tt):
+        """the down path: the encoder output x_l of every level"""
         xs, x = [], x0
-        # transposed tables for the input gradients, built on first use in backward and cached on the hierarchy
-        tt = lambda idx, l: (lambda: transposed_table(svh, idx, svh.num_voxels(l))) if impl == "cuda" else None
         for l in range(D):
             nbr = svh.nbr27[l]
             h = self.enc_a[l](x, nbr, relu=True, idx_t=tt(nbr, l), **kw)
@@ -345,6 +372,25 @@ class SparseUNet(nn.Module):
             xs.append(x)
             if l + 1 < D:
                 x = self.down[l](x, svh.child8[l + 1], relu=True, idx_t=tt(svh.child8[l + 1], l), **kw)
+        return xs
+
+    def _heads(self, out, l, y):
+        C = self.kernel_dim
+        o = self.heads[l](y)
+        out.structure[l], out.normal[l] = o[:, :3], o[:, 3:6]
+        out.basis[l], out.udf[l] = o[:, 6:6 + C], o[:, 6 + C:6 + 2 * C]
+        out.decoder[l] = y
+
+    def forward(self, x0, svh, tf32=False, impl="cuda", grow=None):
+        """the U-Net on the encoder hierarchy `svh`; with `grow` (a dict of `forward_grown`'s keyword arguments) the
+        decoder runs on the hierarchy grown from the structure logits instead"""
+        if grow is not None:
+            return self.forward_grown(x0, svh, tf32=tf32, impl=impl, **grow)
+        D = min(self.depth, svh.depth)
+        kw = dict(tf32=tf32, impl=impl)
+        # transposed tables for the input gradients, built on first use in backward and cached on the hierarchy
+        tt = lambda idx, l: (lambda: transposed_table(svh, idx, svh.num_voxels(l))) if impl == "cuda" else None
+        xs = self._encode(x0, svh, D, kw, tt)
         ys = [None] * D
         y = xs[D - 1]
         ys[D - 1] = y
@@ -359,6 +405,40 @@ class SparseUNet(nn.Module):
             out.structure[l], out.normal[l] = o[:, :3], o[:, 3:6]
             out.basis[l], out.udf[l] = o[:, 6:6 + C], o[:, 6 + C:6 + 2 * C]
             out.decoder[l] = ys[l]
+        return out
+
+    def forward_grown(self, x0, svh, adaptive_depth, forced=None, max_ratio=None, tf32=False, impl="cuda"):
+        """The decoder on the hierarchy T grown from its own structure logits (DESIGN.md SPEC S16).  The down path is
+        `forward`'s.  Going up, level l of T is decoded as y_l = relu(dec_l([skip ; u])) over T.nbr27[l], u the
+        up-projection of y_{l+1} through T's parent-by-octant table and the skip input E's encoder output x_l gathered
+        through skip27 = join_l o T.nbr27[l]; the heads run on y_l at once, and the structure logits of level l (or
+        `forced(T, l)`, the classes of teacher forcing) decide T_{l-1}.
+        Returns the heads and decoder outputs per level on T (structure / normal / basis / udf / decoder), plus
+        `udf_svh` (T), `dec_svh` (the kept voxels), `kept[l]` (indices into T_l of dec_svh's voxels), `classes[l]`
+        and `growth` (the StructureGrowth, with its join and skip tables).  impl='torch' grows with the torch
+        restatement and convolves with the dense-gather torch path."""
+        from .structure import DEFAULT_MAX_RATIO, StructureGrowth
+        D = min(self.depth, svh.depth)
+        kw = dict(tf32=tf32, impl=impl)
+        tt = lambda idx, l: (lambda: transposed_table(svh, idx, svh.num_voxels(l))) if impl == "cuda" else None
+        xs = self._encode(x0, svh, D, kw, tt)
+        g = StructureGrowth(svh, D, adaptive_depth, DEFAULT_MAX_RATIO if max_ratio is None else max_ratio, impl)
+        T = g.T
+        out = SimpleNamespace(structure={}, normal={}, basis={}, udf={}, decoder={})
+        y = xs[D - 1]
+        for l in range(D - 1, -1, -1):
+            if l < D - 1:
+                u = self.up_project(y, T, l, **kw)
+                skip, nbr = g.skip27(l), T.nbr27[l]
+                n_e, n_t = svh.num_voxels(l), T.num_voxels(l)
+                idx_t = ((lambda s=skip, n=n_e: transposed_table(T, s, n)),
+                         (lambda b=nbr, n=n_t: transposed_table(T, b, n))) if impl == "cuda" else None
+                y = self.dec[l]((xs[l], u), (skip, nbr), relu=True, idx_t=idx_t, **kw)
+            self._heads(out, l, y)
+            c = forced(T, l) if forced is not None else None
+            g.step(l, logits=None if c is not None else out.structure[l].detach(), forced=c)
+        out.dec_svh = g.finish()
+        out.udf_svh, out.kept, out.classes, out.growth = T, g.kept, g.classes, g
         return out
 
 

@@ -4,6 +4,7 @@ the structure and UDF losses (nksr_b200/training.py), Adam lr 1e-4, gradient nor
     python tools/train_unet.py --scene sphere --points 200000 --steps 30 --precision fp32 --out ckpt.pt
     python tools/train_unet.py --scene cfg4 --points 1000000 --depth 4 --precision tc --steps 10
     python tools/train_unet.py --scene cfg4 --points 1000000 --depth 4 --kernel-losses --steps 10
+    python tools/train_unet.py --scene cfg4 --points 1000000 --depth 4 --structure predicted --steps 10
 
 Scenes: 'sphere' (tests/clouds.py, exact normals) or 'cfg4' (a crop of bench.py's outdoor scene at its own density,
 normals from the kNN preprocess).  Every step prints one JSON line: the losses and the CUDA-event times of the forward,
@@ -13,6 +14,10 @@ achieved TFLOP/s (2 nnz_taps c_in c_out per call) and GB/s per (c_in, c_out) sha
 --kernel-losses adds the kernel-field losses (GT-surface value / normal, spatial TSDF), trained through the kernel solve,
 and reports them per step with the CUDA-event times of the forward solve (assembly + PCG), the adjoint PCG and the VJP
 kernels (with the field evaluations they need).
+--structure predicted grows the decoder hierarchy from the structure head (teacher-forced from the ground truth, or
+from the prediction with probability --pd-structure-prob); after training one more line reports, per level, the
+structure accuracy and the sizes |E_l| (encoder), |T_l| (grown) and |dec_l| (kept), the CUDA-event time of every growth
+step and the backbone's forward time on the encoder hierarchy against the grown one under teacher forcing.
 --out saves {'state_dict': ...}, which load_checkpoint_from_url(<path>) + load_state_dict take."""
 import argparse
 import json
@@ -89,6 +94,56 @@ class KernelTimer:
                         gbs=round(v["bytes"] / v["ms"] / 1e6, 1)) for k, v in per.items()}
 
 
+def structure_report(net, scene, pd, reps=5):
+    """after training, without grad: per level the structure accuracy (argmax of the logits against the ground truth's
+    voxel status on the hierarchy the decoder predicted for), |E_l|, |T_l| (the grown hierarchy) and |dec_l| (its kept
+    voxels); the CUDA-event time of the growth step of every level; and the median forward time of the backbone
+    (encoder hierarchy vs grown hierarchy under teacher forcing)"""
+    import torch
+    from nksr_b200 import structure as S
+    from nksr_b200.svh import SparseIndexGrid
+    D = min(net.backbone_net.depth, scene.enc_svh.depth)
+    step_ms, orig = {}, S.StructureGrowth.step
+
+    def timed_step(self, l, *a, **k):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        orig(self, l, *a, **k)
+        e1.record()
+        step_ms.setdefault(l, []).append((e0, e1))
+    with torch.no_grad():
+        enc = net.encoder(scene.xyz, scene.normal, scene.enc_svh, 0)
+        gt = None if pd >= 1.0 else scene.gt_svh
+        feat, dec, udf = net.unet(enc, scene.enc_svh, adaptive_depth=scene.adaptive_depth, gt_decoder_svh=gt)
+        acc = {}
+        for l, logits in feat.structure_features.items():
+            if logits.shape[0]:
+                want = scene.gt_svh.evaluate_voxel_status(SparseIndexGrid(udf, l), l)
+                acc[l] = round(float((torch.argmax(logits, dim=1) == want).float().mean()), 4)
+        sizes = [dict(level=l, enc=scene.enc_svh.num_voxels(l), grown=udf.num_voxels(l), dec=dec.num_voxels(l),
+                      accuracy=acc.get(l)) for l in range(D)]
+        times = {}
+        S.StructureGrowth.step = timed_step
+        try:
+            for mode in ("encoder", "predicted"):
+                grow = None if mode == "encoder" else dict(adaptive_depth=scene.adaptive_depth,
+                                                          forced=S.teacher_classes(scene.gt_svh))
+                ms = []
+                for _ in range(reps):
+                    step_ms.clear()
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    net.backbone_net(enc.x0, scene.enc_svh, tf32=net.tf32, grow=grow)
+                    e1.record()
+                    torch.cuda.synchronize()
+                    ms.append(e0.elapsed_time(e1))
+                times[f"backbone_forward_{mode}_ms"] = round(statistics.median(ms), 3)
+        finally:
+            S.StructureGrowth.step = orig
+        growth = {l: round(sum(a.elapsed_time(b) for a, b in v) / len(v), 3) for l, v in sorted(step_ms.items())}
+    return dict(levels=sizes, growth_step_ms=growth, **times)
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--scene", choices=("sphere", "cfg4"), default="sphere")
@@ -99,6 +154,10 @@ def main(argv=None):
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--out", default=None, help="checkpoint path ({'state_dict': ...})")
     ap.add_argument("--kernel-losses", action="store_true", help="add the kernel-field losses (train through the solve)")
+    ap.add_argument("--structure", choices=("encoder", "predicted"), default="encoder",
+                    help="decoder hierarchy: the encoder's, or grown from the structure head (DESIGN.md SPEC S16)")
+    ap.add_argument("--pd-structure-prob", type=float, default=0.0,
+                    help="--structure predicted: probability of growing from the prediction instead of teacher forcing")
     args = ap.parse_args(argv)
     if args.steps < 1:
         ap.error("--steps must be >= 1")
@@ -114,12 +173,13 @@ def main(argv=None):
     dev = torch.device("cuda:0")
     scene = make_scene(args.scene, args.points, args.depth, dev)
     net = NKSRNetwork(dict(backbone="unet", tree_depth=args.depth, kernel_dim=4, precision=args.precision,
-                           trainable=True, seed=args.seed)).to(dev)
+                           trainable=True, seed=args.seed, structure=args.structure)).to(dev)
     opt = T.make_optimizer(net)
     gen = torch.Generator(device=dev).manual_seed(args.seed)
     timer = KernelTimer(U)
     info = dict(gpu_info(0), scene=args.scene, points=int(scene.xyz.shape[0]), voxel_size=scene.voxel_size,
-                depth=args.depth, precision=args.precision,
+                depth=args.depth, precision=args.precision, structure=args.structure,
+                pd_structure_prob=args.pd_structure_prob,
                 voxels=[scene.enc_svh.num_voxels(l) for l in range(args.depth)])
     print(json.dumps(dict(setup=info)), flush=True)
     rows = []
@@ -134,7 +194,8 @@ def main(argv=None):
             timer.phase = {"forward": "backward", "backward": "step"}.get(name, "forward")
         timer.phase = "forward"
         stages = StageTimer(dev, enabled=True) if args.kernel_losses else None
-        out = T.train_step(net, opt, scene, gen, marks, kernel=args.kernel_losses, timer=stages)
+        out = T.train_step(net, opt, scene, gen, marks, kernel=args.kernel_losses, timer=stages,
+                           pd_structure_prob=args.pd_structure_prob)
         l_struct, l_udf = out[:2]
         timer.phase = "forward"
         torch.cuda.synchronize()
@@ -160,6 +221,8 @@ def main(argv=None):
                        "adjoint_pcg_ms", "vjp_ms") if key in timed[0]}
     med["backward_over_forward"] = round(med["backward_ms"] / med["forward_ms"], 3)
     print(json.dumps(dict(summary=med, wgrad_last_step=timer.wgrad_rates(), **info)), flush=True)
+    if args.structure == "predicted":
+        print(json.dumps(dict(structure=structure_report(net, scene, args.pd_structure_prob))), flush=True)
     if args.out:
         torch.save({"state_dict": net.state_dict()}, args.out)
 
