@@ -260,6 +260,7 @@ int nksr_mesh_leaf_flags(const nksr_svh_t* svh, int level, int32_t* flag, void* 
   return NKSR_OK;
 }
 
+// (levels above 6 are refused: 8^7 anchors per leaf; meshing.py MAX_VIRTUAL_LEVEL states the same limit)
 int nksr_mesh_virtual_anchors(const nksr_svh_t* svh, int level, const int32_t* flag, const int64_t* scan,
                               int32_t* anchors, void* stream) {
   if (!svh || level < 1 || level >= svh->depth || level > 6) return NKSR_E_INVALID;

@@ -15,6 +15,7 @@ from . import _lib
 from ._lib import call, stream_ptr
 
 MAX_LATTICE_EXTENT = 1 << 20      # per axis, so that (morton << 2) | axis fits 62 bits
+MAX_VIRTUAL_LEVEL = 6             # coarsest level whose leaves nksr_mesh_virtual_anchors expands (csrc/mesh.cu)
 
 
 class DualMesh(SimpleNamespace):
@@ -71,6 +72,17 @@ def extract_dual_mesh(field, grid_upsample: int = 1, mise_iter: int = 0, max_poi
         # is the cube between 2x2x2 finest voxels, real or virtual -- one lattice, no cracks at level transitions
         if cell_filter is not None:
             raise _lib.NksrError("multi-level meshing does not take a cell filter (multi-GPU meshing)")
+        # leaves above MAX_VIRTUAL_LEVEL (8^7 finest voxels each) are refused before any anchor is allocated
+        for l in range(MAX_VIRTUAL_LEVEL + 1, coarse):
+            if svh.num_voxels(l) == 0:
+                continue
+            leaf = torch.empty(svh.num_voxels(l), dtype=torch.int32, device=dev)
+            call("nksr_mesh_leaf_flags", svh.view(), l, leaf, st)
+            n_leaf = int(leaf.sum().item())
+            if n_leaf:
+                raise _lib.NksrError(f"multi-level meshing expands leaves of levels 1..{MAX_VIRTUAL_LEVEL} only: level "
+                                     f"{l} has {n_leaf} leaves (8^{l} finest voxels each); use adaptive_depth <= "
+                                     f"{MAX_VIRTUAL_LEVEL + 1}")
         anchors = [torch.empty((n0, 3), dtype=torch.int32, device=dev)]
         if n0:
             call("nksr_decode_ijk", svh.keys[0], n0, 0, anchors[0], st)

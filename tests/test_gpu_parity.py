@@ -10,6 +10,7 @@ from oracle import nksr_oracle as O
 from tests import clouds
 from tests.bounds import (KAPPA_FIELD, KAPPA_GRAM, KAPPA_RHS, KAPPA_ROWS, KAPPA_SPMV, assert_within, level_of,
                           level_pair_label)
+from tests.placement_checks import assert_structural_placement
 
 pytestmark = pytest.mark.gpu
 
@@ -259,7 +260,6 @@ def test_structural_placement_is_the_same_matrix(cuda, monkeypatch, L, W, prune)
     (placement_proto.transposed_order), each hold bitwise the entry they copy, and are stored identically run to run."""
     import nksr_b200
     from nksr_b200 import fields
-    from oracle import placement_proto as PP
     monkeypatch.setattr(fields, "BRICK_MIN_LOCATIONS_PER_VOXEL", 0.0)
     xyz, _ = clouds.shapenet_like(3000)
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(cuda)
@@ -273,16 +273,6 @@ def test_structural_placement_is_the_same_matrix(cuda, monkeypatch, L, W, prune)
     nxyz = np.concatenate([osvh.centers(d) for d in range(min(2, L))])
     nval = -(nxyz / np.linalg.norm(nxyz, axis=1, keepdims=True)).astype(np.float32)
     pw, nw = 1e4 / xyz.shape[0], 1e4 / nxyz.shape[0] * W * W
-    pattern = O.structural_pattern(osvh)
-    P = pattern.tocoo()
-    offs = osvh.offsets()
-    n = int(offs[-1])
-    level = lambda i: np.searchsorted(offs, i, side="right") - 1
-    finer = level(P.col) < level(P.row)
-    cnt_ref = np.bincount(P.row[~finer], minlength=n)
-    down_ref = np.bincount(P.row[finer], minlength=n)
-    order_rows, order_cols = PP.transposed_order(osvh)
-    assert order_cols.shape[0] == int(down_ref.sum()) > 0
     for fill in ("rows", "brick"):
         out = []
         for _ in range(2):
@@ -291,24 +281,8 @@ def test_structural_placement_is_the_same_matrix(cuda, monkeypatch, L, W, prune)
             field.solve(t(xyz), t(nxyz), t(nval), pw, nw, 1.0)
             s = field.system
             out.append([_np(a).copy() for a in (s.rowptr, s.col, s.val, s.cnt, s.cnt_down)])
-        (rp, col, val, cnt, cnt_down), again = out
-        # row lengths and pattern: no slot written twice, none left unwritten
-        assert np.array_equal(cnt, cnt_ref) and np.array_equal(cnt_down, down_ref), fill
-        assert np.array_equal(rp, np.concatenate([[0], np.cumsum(cnt_ref + down_ref)])), fill
-        A = sp.csr_matrix((np.ones(col.shape[0]), col, rp), shape=(n, n), copy=True)   # (sum_duplicates sorts in place)
-        A.sum_duplicates()
-        assert A.nnz == rp[-1] and (A - pattern).count_nonzero() == 0, fill
-        # the finer-level segment of every row in the S6b order
-        row_of = np.repeat(np.arange(n), np.diff(rp))
-        down = np.arange(rp[-1]) - rp[row_of] >= cnt[row_of]
-        assert np.array_equal(row_of[down], order_rows) and np.array_equal(col[down], order_cols), fill
-        # every transposed copy (c, j) is bitwise the value row j stores for column c
-        own_key = row_of[~down] * n + col[~down]
-        srt = np.argsort(own_key)
-        src_key = col[down].astype(np.int64) * n + row_of[down]
-        at = np.minimum(np.searchsorted(own_key[srt], src_key), own_key.size - 1)
-        assert np.array_equal(own_key[srt][at], src_key), fill
-        assert np.array_equal(val[~down][srt][at].view(np.uint32), val[down].view(np.uint32)), fill
+        assert_structural_placement(osvh, *out[0], fill)
+        again = out[1]
         for a, b in zip(out[0][:3], again[:3]):
             assert np.array_equal(a, b), fill
 
