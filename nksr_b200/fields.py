@@ -31,8 +31,8 @@ DEFAULT_ROW_LAYOUT = "levels"
 # the Gram fill (solver_config['fill'] or the NKSR_FILL environment variable override it): "brick", "rows", "grouped"
 DEFAULT_FILL = "brick"
 # 'brick' bricks a fine level only when it holds at least this many constraint locations per voxel (measured on H100:
-# faster at 18 per voxel, slower at 1.7 and 4.9; DESIGN 4.1)
-BRICK_MIN_LOCATIONS_PER_VOXEL = 8.0
+# faster than the row fill at 18 per voxel, slower at 1.7, 4.9 and 8.2; DESIGN 4.1)
+BRICK_MIN_LOCATIONS_PER_VOXEL = 12.0
 
 
 _TOTAL_MEMORY = {}

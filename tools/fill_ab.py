@@ -4,13 +4,21 @@ Builds the bench.py system once (cfg4 at 5 M points, seed 4, bench.SOLVER), then
 reconstruct() -- where every buffer of the fill is alive -- times with CUDA events:
   * the row fill (k_gram_fill) on the rows of each level, and on all rows;
   * the brick fill (nksr_gram_fill_brick) on all rows, with the default density threshold and with every level below
-    the split level bricked.
+    the split level bricked;
+  * the brick fill with the threshold set between the levels' densities, so that levels l and up are bricked, for
+    every fine level l: the brick time of level l is the difference of two such fills plus the row fill of level l.
 It prints n per level, the constraint rows per voxel, the kernel-row lines the row fill loads per level (every source
-voxel's lines once per active neighbour row), the GPU name and power limit, and one JSON line.
+voxel's lines once per active neighbour row), the GPU name and power limit, and one JSON line.  With --hash it also
+prints a SHA-256 of each array of the system the brick fill makes with every fine level bricked (rowptr, col, val,
+rhs, diag); with --against LIB, the same for the brick fill of another build of libnksr_b200.so run on the same
+buffers, so that two builds are compared bit for bit on one input (the constraint rows of two runs of reconstruct()
+need not be in the same order).
 
-    python tools/fill_ab.py [--workload cfg4_outdoor_5M] [--reps 3]
+    python tools/fill_ab.py [--workload cfg4_outdoor_5M] [--reps 3] [--hash] [--against path/to/libnksr_b200.so]
 """
 import argparse
+import ctypes
+import hashlib
 import json
 import os
 import subprocess
@@ -36,11 +44,13 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--workload", default="cfg4_outdoor_5M", choices=sorted(bench.WORKLOADS))
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--hash", action="store_true")
+    ap.add_argument("--against", default=None, help="another build's libnksr_b200.so (implies --hash)")
     args = ap.parse_args()
 
     import torch
     import nksr_b200
-    from nksr_b200 import fields
+    from nksr_b200 import _lib, fields
 
     dev = torch.device("cuda", 0)
     cfg = bench.WORKLOADS[args.workload]
@@ -98,6 +108,37 @@ def main():
         result["brick_ms"] = round(ev_time(lambda: orig_call("nksr_gram_fill_brick", *brick_args)), 3)
         result["brick_every_level_ms"] = round(ev_time(lambda: orig_call("nksr_gram_fill_brick",
                                                                           *brick_args[:10], 0.0, st)), 3)
+        # levels >= l bricked: a threshold just under level l's constraint locations per voxel (density grows with l)
+        nsplit = min(int(cs.split_level), L)
+        locations = float(cs.n_pos) + float(cs.n_nrm)
+        dens = [locations / max(offs[l + 1] - offs[l], 1) for l in range(nsplit)]
+        from_level = [ev_time(lambda: orig_call("nksr_gram_fill_brick", *brick_args[:10],
+                                                float(min(dens[l:])) * 0.999, st)) for l in range(nsplit)]
+        from_level.append(result["rows_ms"])
+        result["locations_per_voxel"] = [round(d, 3) for d in dens]
+        result["brick_ms_per_level"] = [round(from_level[l] - from_level[l + 1] + per[l], 3) for l in range(nsplit)]
+        if args.hash or args.against:
+            def hashed(fill):
+                for t in (col, val, rhs, diag):
+                    t.zero_()
+                fill()
+                torch.cuda.synchronize()
+                return {k: hashlib.sha256(t.contiguous().cpu().numpy().tobytes()).hexdigest()
+                        for k, t in (("rowptr", rowptr), ("col", col), ("val", val), ("rhs", rhs), ("diag", diag))}
+            this = lambda: orig_call("nksr_gram_fill_brick", *brick_args[:10], 0.0, st)
+            result["sha256_every_level_bricked"] = hashed(this)
+            if args.against:
+                other = ctypes.CDLL(os.path.abspath(args.against))
+                fn = other.nksr_gram_fill_brick
+                ret, kinds = _lib._SIGNATURES["nksr_gram_fill_brick"]
+                fn.restype = ctypes.c_int
+                fn.argtypes = [_lib._T[k] for k in kinds]
+                conv = [_lib._conv(k, v) for k, v in zip(kinds, brick_args[:10] + (0.0, st))]
+                rcs = []
+                result["sha256_against"] = hashed(lambda: rcs.append(fn(*conv)))
+                result["against_rc"] = rcs[0]
+                result["bitwise_equal"] = result["sha256_against"] == result["sha256_every_level_bricked"]
+                this()                                   # the solve goes on with this build's system
         # counts from the constraint-row ranges
         n_l, pos_per, nrm_per, lines = [], [], [], []
         for l in range(L):
@@ -131,6 +172,7 @@ def main():
     result["gpu"] = gpu_info()
     result["workload"] = args.workload
     result["fill"] = os.environ.get("NKSR_FILL", "default")
+    result["row_layout"] = os.environ.get("NKSR_ROW_LAYOUT", "default")
     if "rows_ms_per_level" in result:
         below = sum(result["rows_ms_per_level"][:max(result["split_level"], 0)])
         result["rows_share_below_split"] = round(below / max(sum(result["rows_ms_per_level"]), 1e-9), 3)
