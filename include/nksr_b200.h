@@ -370,6 +370,19 @@ NKSR_API int nksr_mesh_triangles(const int32_t* mc_case, const int64_t* ekeys12,
 /* LayerField mask (models/nksr_net.py:132): 1 if x lies in an active voxel of level < adaptive_depth */
 NKSR_API int nksr_layer_mask(const nksr_svh_t* svh, const float* xyz, int64_t m, int adaptive_depth,
                     float* out, void* stream);
+/* NeuralField interpolation (models/nksr_net.py:124-130, models/loss.py:120-140; SPEC S17): level_mask = the given
+ * levels (bit l, at least one, all < depth; a given level may be empty, its feat->z[l] is then not read).
+ * out (m x C*popcount(level_mask), every entry written) = per query the trilinear interpolation of feat->z[l] on each
+ * given level in ascending order; 0 where the query has no containing voxel on that level or is non-finite / outside
+ * the key range. */
+NKSR_API int nksr_neural_interp(const nksr_svh_t* svh, const nksr_feat_t* feat, int level_mask, const float* xyz,
+                                int64_t m, float* out, void* stream);
+/* its VJP: xyz = Morton SORTED queries (each with a containing voxel on the coarsest level), range = nksr_row_ranges
+ * of every level concatenated in level order, grad (m x C*popcount(level_mask)) in the same sorted order.  dfeat
+ * (n_total x C, level blocks at svh->offset): the blocks of the given levels are OVERWRITTEN with
+ * sum_q T3(q) grad[q]; the others are not touched.  Deterministic: no atomics, one fixed summation order. */
+NKSR_API int nksr_neural_interp_vjp(const nksr_svh_t* svh, int channels, int level_mask, const float* xyz,
+                                    const int32_t* range, int64_t m, const float* grad, float* dfeat, void* stream);
 
 /* ---- f1: nksr.get_estimate_normal_preprocess_fn (examples/recons_waymo.py:36; CPU twin
  *      examples/recons_waymo_cpu.py:21-41): voxel-neighbourhood PCA normals ---- */

@@ -91,6 +91,30 @@ def _as_level_list(features, depth):
     return [features[d] if d < len(features) else None for d in range(depth)]
 
 
+def _sorted_locations(svh: SparseFeatureHierarchy, xyz: torch.Tensor, extra: Optional[torch.Tensor] = None):
+    """Morton-sort locations and locate them on every level: (perm, sorted xyz, sorted extra, base (depth, m),
+    ranges (n, 2): the first / last + 1 sorted location of every voxel, levels concatenated)."""
+    dev = xyz.device
+    st = stream_ptr(dev)
+    m = xyz.shape[0]
+    status = torch.zeros(1, dtype=torch.int32, device=dev)
+    hk = torch.empty(m, dtype=torch.int64, device=dev)
+    call("nksr_point_half_keys", xyz, m, svh.voxel_size, hk, status, st)
+    if int(status.item()) & 1:
+        raise _lib.NksrError("constraint locations outside the supported range (|x| < 2^19 voxels) or non-finite")
+    _, perm = _lib.sort_pairs(hk, torch.arange(m, dtype=torch.int32, device=dev))
+    perm = perm.long()
+    xs = xyz[perm].contiguous()
+    ex = extra[perm].contiguous() if extra is not None else None
+    base = svh.locate(xs)
+    n_total = svh.num_unknowns
+    ranges = torch.empty((n_total, 2), dtype=torch.int32, device=dev)
+    offs = svh.offsets
+    for l in range(svh.depth):
+        call("nksr_row_ranges", base[l], m, ranges[offs[l]:], svh.num_voxels(l), st)
+    return perm, xs, ex, base, ranges
+
+
 _SIDE_STREAMS = {}
 
 
@@ -166,27 +190,7 @@ class KernelField(BaseField):
 
     # ------------------------------------------------------------------ solve
     def _sorted_locations(self, xyz: torch.Tensor, extra: Optional[torch.Tensor] = None):
-        """Morton-sort locations and locate them on every level: (perm, sorted xyz, sorted extra, base (depth, m),
-        ranges (n, 2): the first / last + 1 sorted location of every voxel, levels concatenated)."""
-        svh, dev = self.svh, xyz.device
-        st = stream_ptr(dev)
-        m = xyz.shape[0]
-        status = torch.zeros(1, dtype=torch.int32, device=dev)
-        hk = torch.empty(m, dtype=torch.int64, device=dev)
-        call("nksr_point_half_keys", xyz, m, svh.voxel_size, hk, status, st)
-        if int(status.item()) & 1:
-            raise _lib.NksrError("constraint locations outside the supported range (|x| < 2^19 voxels) or non-finite")
-        _, perm = _lib.sort_pairs(hk, torch.arange(m, dtype=torch.int32, device=dev))
-        perm = perm.long()
-        xs = xyz[perm].contiguous()
-        ex = extra[perm].contiguous() if extra is not None else None
-        base = svh.locate(xs)
-        n_total = svh.num_unknowns
-        ranges = torch.empty((n_total, 2), dtype=torch.int32, device=dev)
-        offs = svh.offsets
-        for l in range(svh.depth):
-            call("nksr_row_ranges", base[l], m, ranges[offs[l]:], svh.num_voxels(l), st)
-        return perm, xs, ex, base, ranges
+        return _sorted_locations(self.svh, xyz, extra)
 
     def _sorted_rows(self, xyz: torch.Tensor, mode: int, extra: Optional[torch.Tensor] = None,
                      interleaved: bool = False, loc=None):
@@ -652,22 +656,79 @@ class LayerField(BaseField):
 
 
 class NeuralField(BaseField):
-    """MLP-decoded field over trilinearly interpolated voxel features (used as the UDF mask,
-    models/nksr_net.py:124-130).  The decoder is a PyTorch module and stays on PyTorch
-    (north_star: the network is not part of the hot path); interpolation uses the SVH tables."""
+    """MLP-decoded field over trilinearly interpolated voxel features (the UDF mask, models/nksr_net.py:124-130; SPEC
+    S17): f(x) = decoder(u(x)), u(x) = the interpolated features of every given level (a level with features, empty or
+    not) in ascending order, C columns each.  The interpolation and its VJP are CUDA (csrc/neural_field.cu); the
+    decoder is a PyTorch module.  When grad is enabled and the features or the decoder's parameters require grad, the
+    values carry a graph into both (queries get no gradient)."""
 
     def __init__(self, svh: SparseFeatureHierarchy, decoder, features):
         super().__init__(svh)
         self.decoder = decoder
         self.features = _as_level_list(features, svh.depth)
+        given = [l for l, f in enumerate(self.features) if f is not None]
+        if not given:
+            raise ValueError("NeuralField needs features on at least one level")
+        channels = {self.features[l].shape[1] for l in given}
+        if len(channels) != 1:
+            raise ValueError("all given levels must share one feature width")
+        self.channels = channels.pop()
+        if not (1 <= self.channels <= 32):
+            raise ValueError("NeuralField features must have 1..32 channels")
+        for l in given:
+            if self.features[l].shape[0] != svh.num_voxels(l):
+                raise ValueError(f"features[{l}] has {self.features[l].shape[0]} rows but level {l} has "
+                                 f"{svh.num_voxels(l)} voxels")
+        self.levels = given
+        self.level_mask = sum(1 << l for l in given)
+
+    def interpolate(self, xyz: torch.Tensor) -> torch.Tensor:
+        """u(x), (M, C * len(levels)) fp32 (nksr_neural_interp); differentiable in the features when grad is enabled
+        and they require grad"""
+        _lib.require_cuda(xyz, "xyz")
+        xyz = xyz.detach().to(self.svh.device, torch.float32).contiguous()
+        feats = [f.to(self.svh.device, torch.float32).contiguous() if f is not None else None for f in self.features]
+        if torch.is_grad_enabled() and any(f is not None and f.requires_grad for f in feats):
+            return _NeuralInterp.apply(self, xyz, *feats)
+        return self._interp_cuda(xyz, feats)
+
+    def _interp_cuda(self, xyz, feats):
+        m = xyz.shape[0]
+        out = torch.empty((m, self.channels * len(self.levels)), dtype=torch.float32, device=xyz.device)
+        fv = _lib.FeatT()
+        fv.channels = self.channels
+        for l, f in enumerate(feats):
+            fv.z[l] = f.data_ptr() if f is not None and f.shape[0] > 0 else None
+        call("nksr_neural_interp", self.svh.view(), fv, self.level_mask, xyz, m, out, stream_ptr(xyz.device))
+        return out
+
+    def _interp_vjp(self, xyz, g):
+        """dL/dF_l for every level (None where not given) from g = dL/du (nksr_neural_interp_vjp): the queries with a
+        containing voxel are Morton sorted and gathered per voxel, in one fixed order"""
+        svh, dev = self.svh, xyz.device
+        dz = torch.zeros((svh.num_unknowns, self.channels), dtype=torch.float32, device=dev)
+        if svh.num_unknowns > 0 and xyz.shape[0] > 0:
+            keep = torch.nonzero(svh.locate(xyz)[svh.depth - 1] >= 0).reshape(-1)
+            perm, xs, _, _, ranges = _sorted_locations(svh, xyz[keep].contiguous())
+            gs = g.detach().to(torch.float32)[keep[perm]].contiguous()
+            call("nksr_neural_interp_vjp", svh.view(), self.channels, self.level_mask, xs, ranges, xs.shape[0], gs, dz,
+                 stream_ptr(dev))
+        offs = svh.offsets
+        return tuple(dz[offs[l]:offs[l] + svh.num_voxels(l)] if l in self.levels else None for l in range(svh.depth))
 
     def _interp(self, xyz):
+        """plain-torch restatement of `interpolate` (27 masked gathers per level, SPEC S17); a given empty level
+        gives C zero columns"""
         svh = self.svh
         base = svh.locate(xyz).long()
         out = None
         for l in range(svh.depth):
             f = self.features[l]
-            if f is None or svh.num_voxels(l) == 0:
+            if f is None:
+                continue
+            if svh.num_voxels(l) == 0:
+                acc = torch.zeros((xyz.shape[0], f.shape[1]), device=xyz.device, dtype=torch.float32)
+                out = acc if out is None else torch.cat([out, acc], dim=1)
                 continue
             w = svh.voxel_size * (2 ** l)
             b = base[l]
@@ -688,14 +749,36 @@ class NeuralField(BaseField):
         return out
 
     def evaluate_f(self, xyz, grad=False):
-        xyz = xyz.detach().to(self.svh.device, torch.float32).contiguous()
-        with torch.no_grad():
-            v = self.decoder(self._interp(xyz)).reshape(-1)
+        """f at xyz; `gradient` is None (the field has no position gradient here)"""
+        v = self.decoder(self.interpolate(xyz)).reshape(-1)
         return EvaluationResult(value=v, gradient=None)
 
     def mask(self, xyz):
         # UDF semantics: keep geometry closer than the level set to the data
-        return self.evaluate_f(xyz).value <= self.level_set
+        with torch.no_grad():
+            return self.evaluate_f(xyz).value <= self.level_set
+
+    def to_(self, device):
+        super().to_(device)
+        device = torch.device(device)
+        self.features = [f.to(device) if f is not None else None for f in self.features]
+        return self
+
+
+class _NeuralInterp(torch.autograd.Function):
+    """u = interpolate(F, xyz).  Forward: nksr_neural_interp (the same values as without grad).  Backward:
+    dL/dF_l = sum_q T3(q) dL/du_q,l (nksr_neural_interp_vjp); the queries get no gradient."""
+
+    @staticmethod
+    def forward(ctx, field, xyz, *feats):
+        ctx.field, ctx.xyz = field, xyz
+        return field._interp_cuda(xyz, feats)
+
+    @staticmethod
+    def backward(ctx, g):
+        dfeat = ctx.field._interp_vjp(ctx.xyz, g)
+        ctx.field = ctx.xyz = None
+        return (None, None) + tuple(d if need else None for d, need in zip(dfeat, ctx.needs_input_grad[2:]))
 
 
 class SparseFeatureHierarchyCoords:

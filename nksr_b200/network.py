@@ -35,6 +35,8 @@ _DEFAULTS = dict(kernel_dim=4, tree_depth=4, adaptive_depth=2, feature="normal",
                  interpolator=dict(n_hidden=2, hidden_dim=16), udf=dict(enabled=False), seed=0,
                  unet=dict(f_maps=32), backbone="pool", precision="fp32", trainable=False, structure="encoder",
                  structure_max_ratio=None)
+# the UDF decoder of udf.enabled draws its initial weights from seed + this offset
+UDF_DECODER_SEED_OFFSET = 0x5D17
 
 
 def _get(hp, key, default):
@@ -97,6 +99,11 @@ class NKSRNetwork(nn.Module):
         # children a grown level may hold, as a multiple of the encoder voxels of that level (None: the default of
         # nksr_b200/structure.py, DEFAULT_MAX_RATIO)
         self.structure_max_ratio = hp["structure_max_ratio"]
+        # udf.enabled: the mask of a reconstruction is the UDF NeuralField on the decoder hierarchy (DESIGN.md SPEC S17,
+        # models/nksr_net.py:124-130) and training adds its UDF loss over every level -- U-Net backbone only
+        self.udf_enabled = bool(_get(hp["udf"], "enabled", False))
+        if self.udf_enabled and self.backbone != "unet":
+            raise ValueError("udf.enabled needs backbone='unet' (the 'pool' stand-in has no UDF head)")
         interp = hp["interpolator"]
         gen = torch.Generator().manual_seed(int(hp["seed"]))
         state = torch.random.get_rng_state()
@@ -117,6 +124,12 @@ class NKSRNetwork(nn.Module):
                     raise ValueError("unet.f_maps must be a multiple of 32 (csrc/sparse_conv.cu stages 32-channel chunks)")
                 self.point_encoder = PointEncoder(0 if self.feature in (None, "none") else 3, f_maps, f_maps)
                 self.backbone_net = SparseUNet(self.tree_depth, f_maps, C)
+            if self.udf_enabled:
+                # the decoder of u(x), C columns per level; built last from its own seed, so that every other parameter
+                # is bitwise what it is with udf disabled (the Linear(C, 16) above only keeps the draws in step)
+                torch.manual_seed(int(hp["seed"]) + UDF_DECODER_SEED_OFFSET)
+                self.udf_decoder = nn.Sequential(nn.Linear(C * self.tree_depth, 32), nn.ReLU(), nn.Linear(32, 32),
+                                                 nn.ReLU(), nn.Linear(32, 1))
         finally:
             torch.random.set_rng_state(state)
         del gen

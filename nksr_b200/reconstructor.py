@@ -21,7 +21,7 @@ import torch
 
 from . import _lib
 from ._lib import call, stream_ptr
-from .fields import BaseField, EvaluationResult, KernelField, LayerField
+from .fields import BaseField, EvaluationResult, KernelField, LayerField, NeuralField
 from .meshing import DualMesh
 from .network import NKSRNetwork
 from .svh import SparseFeatureHierarchy
@@ -304,6 +304,17 @@ class ChunkedField(BaseField):
         return self
 
 
+def mask_field(network, feats, dec_svh, udf_svh, adaptive_depth: int, voxel_size: float) -> BaseField:
+    """the mask of a reconstruction (models/nksr_net.py:124-133): with udf.enabled the UDF NeuralField over every level
+    of the decoder's udf_svh, keeping f <= 2 voxel_size; else the LayerField of dec_svh's `adaptive_depth` finest
+    levels"""
+    if getattr(network, "udf_enabled", False):
+        nf = NeuralField(udf_svh, network.udf_decoder, feats.udf_features)
+        nf.set_level_set(2.0 * voxel_size)
+        return nf
+    return LayerField(dec_svh, adaptive_depth)
+
+
 class Reconstructor:
     def __init__(self, device, network: Optional[NKSRNetwork] = None, tree_depth: int = 4, adaptive_depth: int = 2,
                  kernel_dim: int = 4):
@@ -337,7 +348,7 @@ class Reconstructor:
         svh = SparseFeatureHierarchy(voxel_size, self.tree_depth, self.device).build_point_splatting(xyz)
         tm.mark("svh_build")
         enc = self.network.encoder(xyz, feat, svh, 0)
-        feats, dec_svh, _ = self.network.unet(enc, svh, adaptive_depth=self.adaptive_depth)
+        feats, dec_svh, udf_svh = self.network.unet(enc, svh, adaptive_depth=self.adaptive_depth)
         if getattr(self.network, "structure", "encoder") == "predicted" and dec_svh.num_unknowns == 0:
             raise _lib.NksrError("predicted structure is empty: the network kept no voxel, there is nothing to solve")
         field = KernelField(dec_svh, self.network.interpolators, feats.basis_features, approx_kernel_grad)
@@ -351,7 +362,7 @@ class Reconstructor:
         normal_weight = NORMAL_WEIGHT / normal_xyz.shape[0] * (voxel_size ** 2)        # models/nksr_net.py:103-104
         field.solve(xyz, normal_xyz, -normal_value, POS_WEIGHT / xyz.shape[0], normal_weight, 1.0,
                     fused_mode=fused_mode)
-        field.set_mask_field(LayerField(dec_svh, ad))
+        field.set_mask_field(mask_field(self.network, feats, dec_svh, udf_svh, ad, voxel_size))
         field._n_normal = int(normal_xyz.shape[0])
         return field
 
@@ -393,6 +404,11 @@ class Reconstructor:
 
     def _reconstruct_chunks(self, xyz, normal, sensor, voxel_size, chunk_size, preprocess_fn, approx_kernel_grad,
                             solver_tol, fused_mode, solver_max_iter, chunk_filter=None):
+        if getattr(self.network, "udf_enabled", False):
+            # (also reached from dist.reconstruct_distributed) the blended field has no UDF hierarchy to mask with
+            raise _lib.NksrError("chunk mode does not support udf.enabled: the blended chunk field has no UDF "
+                                 "hierarchy; build the network with udf=dict(enabled=False) or reconstruct without "
+                                 "chunk_size")
         self._timer = _lib.StageTimer(self.device, enabled=False)
         margin = voxel_size * (2 ** (self.tree_depth - 1)) * 2.0       # two coarsest voxels of overlap
         cidx = torch.floor(xyz / chunk_size).long()

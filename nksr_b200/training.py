@@ -7,6 +7,7 @@ and :106-140), with the samplers and ground-truth transform of configs/default/t
     feat, dec_svh, _ = net.unet(net.encoder(xyz, normal, svh, 0), svh)
     l_struct, per_level = structure_loss(feat.structure_features, dec_svh, gt_svh)
     l_udf = udf_loss(net.udf_decoder, feat.udf_features, dec_svh, ref_xyz, ref_normal, voxel_size)
+    (with udf.enabled: udf_field_loss, the same loss on the NeuralField over every level)
 
 Both are plain torch on top of the hierarchy's CUDA tables; the gradients flow into the network through the sparse
 convolution's backward kernels (nksr_b200/unet.py, csrc/sparse_conv_bwd.cu).
@@ -121,6 +122,19 @@ def udf_loss(udf_decoder, udf_features, svh: SparseFeatureHierarchy, ref_xyz, re
     return torch.mean((transform_field(pd, voxel_size, gt_band) - gt).abs()) / voxel_size
 
 
+def udf_field_loss(udf_decoder, udf_features, svh: SparseFeatureHierarchy, ref_xyz, ref_normal, voxel_size,
+                   samplers=UDF_SAMPLERS, gt_band=GT_BAND, generator=None, q=None):
+    """the UDF loss of udf.enabled (models/loss.py:120-140): the same samples, ground truth and L1 as `udf_loss`, but pd
+    is the UDF NeuralField over every level of `svh` (the decoder takes kernel_dim columns per level), evaluated and
+    backpropagated through the interpolation kernels (csrc/neural_field.cu)"""
+    if q is None:
+        q = udf_samples(svh, ref_xyz, ref_normal, voxel_size, samplers, generator)
+    gt = udf_gt(q, ref_xyz, ref_normal, voxel_size, gt_band)
+    field = NeuralField(svh, udf_decoder, udf_features)
+    pd = field.evaluate_f(q.to(torch.float32).contiguous()).value
+    return torch.mean((transform_field(pd, voxel_size, gt_band) - gt).abs()) / voxel_size
+
+
 class TrainingScene:
     """one oriented cloud with its encoder hierarchy (point splatting) and ground-truth hierarchy (adaptive, from the
     normals, models/nksr_net.py:175-179).  The decoder runs on the encoder hierarchy: the predicted-structure regime,
@@ -213,8 +227,9 @@ def losses(net, scene: TrainingScene, generator=None, kernel=False, timer=None, 
     else:
         feat, dec_svh, udf_svh = net.unet(enc, scene.enc_svh, adaptive_depth=scene.adaptive_depth)
     l_struct, _ = structure_loss(feat.structure_features, udf_svh, scene.gt_svh)
-    l_udf = udf_loss(net.udf_decoder, feat.udf_features, udf_svh, scene.xyz, scene.normal, scene.voxel_size,
-                     generator=generator)
+    loss_fn = udf_field_loss if getattr(net, "udf_enabled", False) else udf_loss
+    l_udf = loss_fn(net.udf_decoder, feat.udf_features, udf_svh, scene.xyz, scene.normal, scene.voxel_size,
+                    generator=generator)
     total = STRUCTURE_WEIGHT * l_struct + UDF_WEIGHT * l_udf
     if not kernel:
         return total, l_struct, l_udf
