@@ -37,6 +37,28 @@ struct PcgCtrl {
   double gamma_prev, alpha_prev;  // Chronopoulos-Gear recurrences (distributed solve)
 };
 
+// sum of val[p] * x[col[p]] over the entries of one row, in every lane of the warp.  The matrix stream: evict-first
+// loads (read once per SpMV); x: read-only path, stays in L1/L2.  Four independent 128 B column + value requests per
+// lane keep ~1 KB per warp in flight.
+__device__ __forceinline__ float row_dot(const int64_t* __restrict__ rowptr, const int32_t* __restrict__ col,
+                                         const float* __restrict__ val, const float* __restrict__ x, int64_t row,
+                                         int lane) {
+  const int64_t b = __ldg(rowptr + row), e = __ldg(rowptr + row + 1);
+  float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
+  for (int64_t p = b + lane; p < e; p += 128) {   // predicated tail: absent entries read as (col 0, value 0)
+    const bool q1 = p + 32 < e, q2 = p + 64 < e, q3 = p + 96 < e;
+    const int c0 = __ldcs(col + p), c1 = q1 ? __ldcs(col + p + 32) : 0, c2 = q2 ? __ldcs(col + p + 64) : 0,
+              c3 = q3 ? __ldcs(col + p + 96) : 0;
+    const float v0 = __ldcs(val + p), v1 = q1 ? __ldcs(val + p + 32) : 0.f, v2 = q2 ? __ldcs(val + p + 64) : 0.f,
+                v3 = q3 ? __ldcs(val + p + 96) : 0.f;
+    s0 = fmaf(v0, __ldg(x + c0), s0);
+    s1 = fmaf(v1, __ldg(x + c1), s1);
+    s2 = fmaf(v2, __ldg(x + c2), s2);
+    s3 = fmaf(v3, __ldg(x + c3), s3);
+  }
+  return warp_sum((s0 + s1) + (s2 + s3));
+}
+
 // y = A x, one warp per row, grid-stride over rows.  DOT: also partial[blockIdx] = sum x_i * y_i.
 // ctrl (nullable): no-op once the solve is over.
 template <bool DOT>
@@ -51,25 +73,9 @@ k_spmv(const int64_t* __restrict__ rowptr, const int32_t* __restrict__ col, cons
   const int64_t nwarps = (int64_t)gridDim.x * kWarpsPerBlock;
   double local = 0.0;
   for (int64_t row = blockIdx.x * (int64_t)kWarpsPerBlock + wid; row < n; row += nwarps) {
-    const int64_t b = __ldg(rowptr + row), e = __ldg(rowptr + row + 1);
     // (prefetching the next row's pointers was tried and measured slower -- the two loop-carried 64-bit
     // values push the kernel past the 32 registers that keep the persistent 8-blocks-per-SM grid resident)
-    // matrix stream: evict-first loads (read once per SpMV); x: read-only path, stays in L1/L2.
-    // Four independent 128 B column + value requests per lane keep ~1 KB per warp in flight.
-    float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-    int64_t p = b + lane;
-    for (; p < e; p += 128) {   // predicated tail: absent entries read as (col 0, value 0)
-      const bool q1 = p + 32 < e, q2 = p + 64 < e, q3 = p + 96 < e;
-      const int c0 = __ldcs(col + p), c1 = q1 ? __ldcs(col + p + 32) : 0, c2 = q2 ? __ldcs(col + p + 64) : 0,
-                c3 = q3 ? __ldcs(col + p + 96) : 0;
-      const float v0 = __ldcs(val + p), v1 = q1 ? __ldcs(val + p + 32) : 0.f, v2 = q2 ? __ldcs(val + p + 64) : 0.f,
-                  v3 = q3 ? __ldcs(val + p + 96) : 0.f;
-      s0 = fmaf(v0, __ldg(x + c0), s0);
-      s1 = fmaf(v1, __ldg(x + c1), s1);
-      s2 = fmaf(v2, __ldg(x + c2), s2);
-      s3 = fmaf(v3, __ldg(x + c3), s3);
-    }
-    float s = warp_sum((s0 + s1) + (s2 + s3));
+    const float s = row_dot(rowptr, col, val, x, row, lane);
     if (lane == 0) {
       y[row] = s;
       if (DOT) local += (double)s * (double)__ldg(x + row);
@@ -424,14 +430,8 @@ int nksr_spmv_stream(const int64_t* rowptr, const int32_t* col, const float* val
     const int rc = spmv_stream_launch(rowptr, col, val, x, y, plan, nullptr, s);
     if (rc != NKSR_OK) return rc;
   }
-  if (split_row < n) {
-    int grid = (int)((n - split_row + kWarpsPerBlock - 1) / kWarpsPerBlock);
-    if (grid > kGrid) grid = kGrid;
-    k_spmv<false><<<grid, kBlock, 0, s>>>(rowptr + split_row, col, val, x, y + split_row, n - split_row, nullptr,
-                                          nullptr);
-    NKSR_CHECK_LAUNCH();
-  }
-  return NKSR_OK;
+  // the rows after the streamed ones: the row kernel
+  return split_row < n ? nksr_spmv(rowptr + split_row, col, val, x, y + split_row, n - split_row, stream) : NKSR_OK;
 }
 
 }  // extern "C"
@@ -457,20 +457,7 @@ k_dcg_spmv(const int64_t* __restrict__ rowptr, const int32_t* __restrict__ col, 
       if (lane == 0) w[row] = 0.f;
       continue;
     }
-    const int64_t b = __ldg(rowptr + row), e = __ldg(rowptr + row + 1);
-    float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-    for (int64_t p = b + lane; p < e; p += 128) {
-      const bool q1 = p + 32 < e, q2 = p + 64 < e, q3 = p + 96 < e;
-      const int c0 = __ldcs(col + p), c1 = q1 ? __ldcs(col + p + 32) : 0, c2 = q2 ? __ldcs(col + p + 64) : 0,
-                c3 = q3 ? __ldcs(col + p + 96) : 0;
-      const float v0 = __ldcs(val + p), v1 = q1 ? __ldcs(val + p + 32) : 0.f, v2 = q2 ? __ldcs(val + p + 64) : 0.f,
-                  v3 = q3 ? __ldcs(val + p + 96) : 0.f;
-      s0 = fmaf(v0, __ldg(u + c0), s0);
-      s1 = fmaf(v1, __ldg(u + c1), s1);
-      s2 = fmaf(v2, __ldg(u + c2), s2);
-      s3 = fmaf(v3, __ldg(u + c3), s3);
-    }
-    const float s = warp_sum((s0 + s1) + (s2 + s3));
+    const float s = row_dot(rowptr, col, val, u, row, lane);
     if (lane == 0) {
       w[row] = s;
       const double ri = (double)__ldg(r + row), ui = (double)__ldg(u + row);
