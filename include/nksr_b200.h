@@ -255,20 +255,38 @@ NKSR_API int nksr_pcg_solve(const int64_t* rowptr, const int32_t* col, const flo
  * into tiles of 4096 entries that one elected thread per CTA moves into a shared-memory ring with bulk async copies
  * (cp.async.bulk + mbarrier); consumer warps form the products in place and reduce the rows from shared memory.  Same
  * result up to the summation order inside a row (fixed, reproducible).  Bulk copies move whole 16-byte units: rowptr
- * must be readable up to index n + 1 (n + 2 entries) and col / val up to the next multiple of 4 entries. */
+ * must be readable up to index n + 1 (n + 2 entries) and col / val up to the next multiple of 4 entries.  The
+ * workspace holds the stream's plan, with room for packed column tiles (nksr_spmv_plan_build): about 2 bytes per
+ * nonzero. */
 NKSR_API size_t nksr_pcg_stream_workspace_bytes(int64_t n, int64_t nnz);
-/* rows [0, split_row) -- entries [0, split_nnz), split_nnz = rowptr[split_row] -- are streamed; rows >= split_row (the
- * coarse levels, whose transposed segments make rows of tens of thousands of entries) go through the warp-per-row
- * kernel, where a long row streams well and does not stall a tile behind one warp.  split_row = n streams everything. */
+/* rows [0, split_row) -- entries [0, split_nnz), split_nnz = rowptr[split_row] -- are streamed; rows >= split_row go
+ * through the warp-per-row kernel.  split_row = n streams everything (what KernelField does: on the H100 the coarse
+ * levels' long rows stream faster as tiles too). */
 NKSR_API int nksr_pcg_solve_stream(const int64_t* rowptr, const int32_t* col, const float* val, const float* diag,
                           const float* b, float* x, int64_t n, int64_t nnz, int64_t split_row, int64_t split_nnz,
                           float tol, int max_iter, int check_every, int profile, void* ws, size_t ws_bytes,
                           double* info, void* stream);
-/* y = A x through the same tile stream (plan_buf: nksr_spmv_plan_bytes(nnz) bytes of scratch) */
+/* y = A x through the same tile stream (plan_buf: nksr_spmv_plan_bytes(nnz) bytes of scratch); builds the plan
+ * (nksr_spmv_plan_build) and runs it (nksr_spmv_stream_planned) */
 NKSR_API size_t nksr_spmv_plan_bytes(int64_t nnz);
 NKSR_API int nksr_spmv_stream(const int64_t* rowptr, const int32_t* col, const float* val, const float* x, float* y,
                      int64_t n, int64_t nnz, int64_t split_row, int64_t split_nnz, void* plan_buf,
                      size_t plan_bytes, void* stream);
+/* the plan of a tile stream: tile boundaries, and room for packed column tiles.  The first SpMV over the plan packs
+ * every tile whose columns lie in at most 8 aligned windows of 8192 columns into window bases plus one uint16 per
+ * entry (3-bit window, 13-bit offset); later SpMVs stream 2 bytes per column of such a tile instead of 4.  Valid
+ * while rowptr and col are unchanged. */
+NKSR_API int nksr_spmv_plan_build(const int64_t* rowptr, int64_t n, int64_t nnz, int64_t split_row, int64_t split_nnz,
+                         void* plan_buf, size_t plan_bytes, void* stream);
+/* out[4] (host) = packed tiles, entries in packed tiles, streamed tiles, streamed entries of a plan that has run at
+ * least one SpMV (the PCG's plan starts nksr_pcg_workspace_bytes(n) bytes into its workspace); synchronises the
+ * stream */
+NKSR_API int nksr_spmv_plan_stats(const void* plan_buf, int64_t* out, void* stream);
+/* y = A x with a plan built by nksr_spmv_plan_build for the same rowptr, col, split_row and split_nnz.  The first
+ * launch over a plan writes it (packed slots, headers, counts): a plan belongs to one stream at a time. */
+NKSR_API int nksr_spmv_stream_planned(const int64_t* rowptr, const int32_t* col, const float* val, const float* x,
+                             float* y, int64_t n, int64_t nnz, int64_t split_row, int64_t split_nnz,
+                             void* plan_buf, void* stream);
 
 /* ---- e: step kernels of the multi-GPU solve (one global system, SURVEY section 8e mapping B).  A
  * Chronopoulos-Gear arrangement of the same Jacobi-PCG: per iteration ONE halo exchange of u = M^-1 r, one

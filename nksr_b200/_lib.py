@@ -93,6 +93,9 @@ _SIGNATURES = {
     "nksr_pcg_solve_stream": ("i", "pppppp" + "qqqqfiii" + "pzdp"),
     "nksr_spmv_plan_bytes": ("z", "q"),
     "nksr_spmv_stream": ("i", "ppppp" + "qqqq" + "pzp"),
+    "nksr_spmv_plan_build": ("i", "p" + "qqqq" + "pzp"),
+    "nksr_spmv_plan_stats": ("i", "ppp"),
+    "nksr_spmv_stream_planned": ("i", "ppppp" + "qqqq" + "pp"),
     "nksr_dcg_workspace_bytes": ("z", ""),
     "nksr_dcg_init": ("i", "pppppppp" + "q" + "pz" + "pp"),
     "nksr_dcg_begin": ("i", "ppfip"),

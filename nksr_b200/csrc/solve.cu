@@ -399,10 +399,12 @@ int nksr_pcg_solve_stream(const int64_t* rowptr, const int32_t* col, const float
   if (n <= 0 || nnz <= 0 || split_row < 0 || split_row > n || split_nnz < 0 || split_nnz > nnz) return NKSR_E_INVALID;
   if (ws_bytes < nksr_pcg_stream_workspace_bytes(n, nnz)) return NKSR_E_WORKSPACE;
   const size_t base = nksr_pcg_workspace_bytes(n);
+  SpmvPlan plan = spmv_plan_carve(reinterpret_cast<unsigned char*>(ws) + base, split_row, split_nnz);
+  if (cudaMemsetAsync(plan.stats, 0, 4 * sizeof(unsigned long long), as_stream(stream)) != cudaSuccess)
+    return NKSR_E_CUDA;
   if (split_row == 0 || split_nnz == 0)     // nothing to stream: the plain solver
     return pcg_solve_impl(rowptr, col, val, diag, b, x, n, tol, max_iter, check_every, profile, ws, base, info, stream,
                           nullptr);
-  SpmvPlan plan = spmv_plan_carve(reinterpret_cast<unsigned char*>(ws) + base, split_row, split_nnz);
   if (spmv_stream_prepare() != NKSR_OK || spmv_stream_sm_count() <= 0) return NKSR_E_CUDA;
   if (spmv_plan_build(rowptr, plan, as_stream(stream)) != NKSR_OK) return NKSR_E_CUDA;
   return pcg_solve_impl(rowptr, col, val, diag, b, x, n, tol, max_iter, check_every, profile, ws, base, info, stream,
@@ -411,12 +413,33 @@ int nksr_pcg_solve_stream(const int64_t* rowptr, const int32_t* col, const float
 
 size_t nksr_spmv_plan_bytes(int64_t nnz) { return spmv_plan_bytes(nnz > 0 ? nnz : 1); }
 
-int nksr_spmv_stream(const int64_t* rowptr, const int32_t* col, const float* val, const float* x, float* y, int64_t n,
-                     int64_t nnz, int64_t split_row, int64_t split_nnz, void* plan_buf, size_t plan_bytes,
-                     void* stream) {
+int nksr_spmv_plan_build(const int64_t* rowptr, int64_t n, int64_t nnz, int64_t split_row, int64_t split_nnz,
+                         void* plan_buf, size_t plan_bytes, void* stream) {
   if (n <= 0 || nnz <= 0 || !plan_buf || split_row < 0 || split_row > n || split_nnz < 0 || split_nnz > nnz)
     return NKSR_E_INVALID;
   if (plan_bytes < spmv_plan_bytes(nnz)) return NKSR_E_WORKSPACE;
+  cudaStream_t s = as_stream(stream);
+  SpmvPlan plan = spmv_plan_carve(plan_buf, split_row, split_nnz);
+  if (cudaMemsetAsync(plan.stats, 0, 4 * sizeof(unsigned long long), s) != cudaSuccess) return NKSR_E_CUDA;
+  if (split_row == 0 || split_nnz == 0) return NKSR_OK;
+  return spmv_plan_build(rowptr, plan, s);
+}
+
+int nksr_spmv_plan_stats(const void* plan_buf, int64_t* out, void* stream) {
+  if (!plan_buf || !out) return NKSR_E_INVALID;
+  cudaStream_t s = as_stream(stream);
+  unsigned long long h[4];
+  if (cudaMemcpyAsync(h, plan_buf, sizeof(h), cudaMemcpyDeviceToHost, s) != cudaSuccess) return NKSR_E_CUDA;
+  if (cudaStreamSynchronize(s) != cudaSuccess) return NKSR_E_CUDA;
+  for (int i = 0; i < 4; ++i) out[i] = (int64_t)h[i];
+  return NKSR_OK;
+}
+
+int nksr_spmv_stream_planned(const int64_t* rowptr, const int32_t* col, const float* val, const float* x, float* y,
+                             int64_t n, int64_t nnz, int64_t split_row, int64_t split_nnz, void* plan_buf,
+                             void* stream) {
+  if (n <= 0 || nnz <= 0 || !plan_buf || split_row < 0 || split_row > n || split_nnz < 0 || split_nnz > nnz)
+    return NKSR_E_INVALID;
   cudaStream_t s = as_stream(stream);
   // the streamed part writes every row of [0, split_row), empty ones included; when those rows hold no entry at all,
   // nothing is streamed and they are zeroed here
@@ -424,14 +447,21 @@ int nksr_spmv_stream(const int64_t* rowptr, const int32_t* col, const float* val
       cudaMemsetAsync(y, 0, (size_t)split_row * sizeof(float), s) != cudaSuccess)
     return NKSR_E_CUDA;
   if (split_row > 0 && split_nnz > 0) {
-    SpmvPlan plan = spmv_plan_carve(plan_buf, split_row, split_nnz);
+    const SpmvPlan plan = spmv_plan_carve(plan_buf, split_row, split_nnz);
     if (spmv_stream_prepare() != NKSR_OK) return NKSR_E_CUDA;
-    if (spmv_plan_build(rowptr, plan, s) != NKSR_OK) return NKSR_E_CUDA;
     const int rc = spmv_stream_launch(rowptr, col, val, x, y, plan, nullptr, s);
     if (rc != NKSR_OK) return rc;
   }
   // the rows after the streamed ones: the row kernel
   return split_row < n ? nksr_spmv(rowptr + split_row, col, val, x, y + split_row, n - split_row, stream) : NKSR_OK;
+}
+
+int nksr_spmv_stream(const int64_t* rowptr, const int32_t* col, const float* val, const float* x, float* y, int64_t n,
+                     int64_t nnz, int64_t split_row, int64_t split_nnz, void* plan_buf, size_t plan_bytes,
+                     void* stream) {
+  const int rc = nksr_spmv_plan_build(rowptr, n, nnz, split_row, split_nnz, plan_buf, plan_bytes, stream);
+  if (rc != NKSR_OK) return rc;
+  return nksr_spmv_stream_planned(rowptr, col, val, x, y, n, nnz, split_row, split_nnz, plan_buf, stream);
 }
 
 }  // extern "C"

@@ -250,22 +250,24 @@ class KernelField(BaseField):
         alpha = torch.empty(n, dtype=torch.float32, device=dev)
         info = (C.c_double * 8)()
         profile = int(bool(self.solver_config.get("profile")))
-        # 'rows' (default): one warp per row with register loads (csrc/solve.cu); 'stream': the CSR arrays reach the SMs
-        # as tiles moved by bulk async copies (TMA engine) into a shared-memory ring (csrc/spmv_stream.cuh)
-        spmv = self.solver_config.get("spmv") or os.environ.get("NKSR_SPMV") or "rows"
+        # 'stream' (default): the CSR arrays reach the SMs as tiles moved by bulk async copies (TMA engine) into a
+        # shared-memory ring, with packed column tiles (csrc/spmv_stream.cuh); 'rows': one warp per row with register
+        # loads (csrc/solve.cu), the reference the stream is tested against
+        spmv = self.solver_config.get("spmv") or os.environ.get("NKSR_SPMV") or "stream"
         if spmv not in ("stream", "rows"):
             raise ValueError("solver_config['spmv'] must be 'stream' or 'rows'")
+        packed = None
         if spmv == "stream":
             nb = call("nksr_pcg_stream_workspace_bytes", n, sysm.nnz)
             ws = torch.empty(nb, dtype=torch.uint8, device=dev)
-            # rows of the two finest levels are streamed; the coarse rows (transposed segments of up to tens of
-            # thousands of entries) go warp per row, where a long row streams well and cannot hold a tile up
-            offs = self.svh.offsets
-            split_row = offs[2] if self.svh.depth > 2 else n
-            split_nnz = int(sysm.rowptr[split_row].item()) if split_row < n else sysm.nnz
+            # every row is streamed: the coarse rows too (transposed segments of up to tens of thousands of
+            # entries), which on the H100 stream faster as tiles than warp per row (DESIGN 4.2)
             call("nksr_pcg_solve_stream", sysm.rowptr, sysm.col, sysm.val, sysm.diag, rhs, alpha, n, sysm.nnz,
-                 split_row, split_nnz, float(self.solver_config["tol"]), int(self.solver_config["max_iter"]),
+                 n, sysm.nnz, float(self.solver_config["tol"]), int(self.solver_config["max_iter"]),
                  int(self.solver_config["check_every"]), profile, ws, nb, info, stream_ptr(dev))
+            packed = (C.c_int64 * 4)()
+            call("nksr_spmv_plan_stats", ws[call("nksr_pcg_workspace_bytes", n):], C.addressof(packed),
+                 stream_ptr(dev))
         else:
             nb = call("nksr_pcg_workspace_bytes", n)
             ws = torch.empty(nb, dtype=torch.uint8, device=dev)
@@ -279,6 +281,9 @@ class KernelField(BaseField):
         else:
             self.solve_info = {"iterations": int(info[0]), "relative_residual": float(info[1]), "n": n,
                                "nnz": sysm.nnz, "converged": status == 0}
+            if packed is not None:
+                self.solve_info.update(spmv_packed_tiles=packed[0], spmv_packed_entries=packed[1],
+                                       spmv_streamed_tiles=packed[2], spmv_streamed_entries=packed[3])
         what = "adjoint PCG" if adjoint else "PCG"
         if status == 2:
             raise _lib.NksrError(f"{what} broke down (non-finite residual) after {int(info[0])} iterations: the system "
