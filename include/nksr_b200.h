@@ -452,6 +452,24 @@ NKSR_API int nksr_sdf_from_points(const nksr_svh_t* svh, const float* xyz, const
                          int nb_points, float stdv, int imls, int start_level, float* sdf, float* grad,
                          void* stream);
 
+/* ---- metrics.MeshEvaluator (models/nksr_net.py:298-312; DESIGN.md SPEC S18).
+ * nksr_sample_surface: n area-uniform samples of the mesh (v: float[V*3], f: int32[n_tri*3]).  start: int64[n_tri+1],
+ * the first sample of every triangle (start[0] = 0, start[n_tri] = n, non-decreasing; the caller forms it from the
+ * fp64 area prefix).  Sample i lies on triangle out_tri[i] at the barycentrics of a counter hash of (seed, i);
+ * out_normal[i] is that triangle's unit normal.
+ * nksr_metric_nearest: for every query, the distance to its nearest point of the Morton-sorted cloud xyz (n_pts >= 1,
+ * hashed as for nksr_nearest_point: svh / range / origin3), that point's index in sorted order (ties: the lower
+ * index) and, when normal, query_normal and out_dot are all given, |n_q . n_t| of the unit normals.  Exact for
+ * every query: those the hierarchy does not resolve are compacted into far_list (int32[m]; *far_count their number,
+ * device int32) and answered by a branch-and-bound over the top-level cells, whose point boxes go to box
+ * (float[6 * svh->n[depth-1]], workspace). */
+NKSR_API int nksr_sample_surface(const float* v, const int32_t* f, int64_t n_tri, const int64_t* start, int64_t n,
+                        int64_t seed, float* out_xyz, float* out_normal, int32_t* out_tri, void* stream);
+NKSR_API int nksr_metric_nearest(const nksr_svh_t* svh, const float* xyz, const float* normal, const int32_t* range,
+                        float* box, int64_t n_pts, const float* query, const float* query_normal, int64_t m,
+                        const float* origin3, int start_level, float* out_dist, int32_t* out_idx, float* out_dot,
+                        int32_t* far_list, int32_t* far_count, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -135,6 +135,8 @@ _SIGNATURES = {
     "nksr_nearest_point": ("i", "Sppqpqpippp"),
     "nksr_knn_mean_distance": ("i", "Sppqppqiipp"),
     "nksr_sdf_from_points": ("i", "Sppppqppqifiippp"),
+    "nksr_sample_surface": ("i", "ppqpqqpppp"),
+    "nksr_metric_nearest": ("i", "Spppp" + "qppqpi" + "pppppp"),
 }
 
 _lib = None

@@ -1,0 +1,195 @@
+"""Mesh-quality metrics -- host mirror of the reference's metrics.MeshEvaluator.
+
+Reference contract:
+  MeshEvaluator(n_points=5e6 or 5e5, metric_names=MeshEvaluator.ESSENTIAL_METRICS)   models/nksr_net.py:298-312
+  .eval_mesh(mesh, ref_xyz, ref_normal, onet_samples=None) -> {name: value}
+
+The mesh is sampled area-uniformly (csrc/metrics.cu: k_sample_surface) and both nearest-neighbour passes are exact
+(k_metric_nearest on the multi-level voxel hash, k_metric_far for the queries the hierarchy does not resolve); the
+means and threshold fractions are fp64 reductions in torch.  DESIGN.md SPEC S18 defines every step.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import logging
+import math
+from typing import Optional
+
+import numpy as np
+import torch
+
+from ._lib import MAX_DEPTH, NksrError, call, require_cuda, stream_ptr
+
+_log = logging.getLogger(__name__)
+
+THRESHOLDS = (0.01, 0.015, 0.02, 0.002, 0.1)
+START_LEVEL = 2         # first level of the nearest-point search, as for PCNNField
+_NAN = float("nan")
+
+
+def _as_tensor(a, device, dtype) -> torch.Tensor:
+    if isinstance(a, torch.Tensor):
+        return a.detach().to(device=device, dtype=dtype).contiguous()
+    return torch.from_numpy(np.ascontiguousarray(np.asarray(a))).to(device=device, dtype=dtype).contiguous()
+
+
+def sample_surface(v: torch.Tensor, f: torch.Tensor, n: int, seed: int = 0):
+    """n area-uniform samples of the triangle mesh (v, f) on its device: (xyz (n, 3), unit triangle normal (n, 3),
+    source triangle (n,) int32).  Triangle t receives the samples [round(n S_{t-1} / A), round(n S_t / A)) of the fp64
+    area prefix S (A = S_T); a mesh without area gives none."""
+    require_cuda(v, "v")
+    dev = v.device
+    v = v.detach().to(torch.float32).contiguous()
+    f = f.detach().to(device=dev, dtype=torch.int32).reshape(-1, 3).contiguous()
+    n = int(n)
+    t = f.shape[0]
+    if t:
+        vd = v.double()
+        area = 0.5 * torch.linalg.vector_norm(torch.linalg.cross(vd[f[:, 1].long()] - vd[f[:, 0].long()],
+                                                                  vd[f[:, 2].long()] - vd[f[:, 0].long()]), dim=1)
+        prefix = torch.cumsum(area, 0)
+        total = float(prefix[-1].item())
+    if n <= 0 or t == 0 or not total > 0.0:
+        return (torch.empty((0, 3), dtype=torch.float32, device=dev), torch.empty((0, 3), dtype=torch.float32, device=dev),
+                torch.empty(0, dtype=torch.int32, device=dev))
+    start = torch.zeros(t + 1, dtype=torch.int64, device=dev)
+    start[1:] = torch.round(n * prefix / total).long().clamp_(0, n)
+    start[-1] = n
+    xyz = torch.empty((n, 3), dtype=torch.float32, device=dev)
+    nrm = torch.empty((n, 3), dtype=torch.float32, device=dev)
+    tri = torch.empty(n, dtype=torch.int32, device=dev)
+    seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+    call("nksr_sample_surface", v, f, t, start, n, seed - (1 << 64) if seed >= 1 << 63 else seed, xyz, nrm, tri,
+         stream_ptr(dev))
+    return xyz, nrm, tri
+
+
+def nearest_neighbours(query: torch.Tensor, target: torch.Tensor, query_normal: Optional[torch.Tensor] = None,
+                       target_normal: Optional[torch.Tensor] = None):
+    """Exact nearest target point of every query: (distance (m,) fp32, index into `target` (m,) int64, |n_q . n_t| of the
+    unit normals (m,), NaN unless both normal sets are given).  Ties go to the lower index of the hash's sorted order,
+    which for coincident target points is their input order.  An empty target gives distance inf and index -1."""
+    from .reconstructor import _knn_hash
+    require_cuda(target, "target")
+    dev = target.device
+    target = target.detach().to(torch.float32).contiguous()
+    query = query.detach().to(dev, torch.float32).contiguous()
+    m, n = query.shape[0], target.shape[0]
+    dot = torch.full((m,), _NAN, dtype=torch.float32, device=dev)
+    if n == 0 or m == 0:
+        return (torch.full((m,), math.inf, dtype=torch.float32, device=dev),
+                torch.full((m,), -1, dtype=torch.int64, device=dev), dot)
+    origin = torch.minimum(target.min(dim=0).values, query.min(dim=0).values)
+    perm, svh, _, ranges, origin = _knn_hash(target, levels=MAX_DEPTH, origin=origin)
+    xs = target[perm].contiguous()
+    both = query_normal is not None and target_normal is not None
+    tn = target_normal.detach().to(dev, torch.float32)[perm].contiguous() if both else None
+    qn = query_normal.detach().to(dev, torch.float32).contiguous() if both else None
+    origin_host = (C.c_float * 3)(*[float(x) for x in origin.tolist()])
+    box = torch.empty((svh.num_voxels(svh.depth - 1), 6), dtype=torch.float32, device=dev)
+    far_list = torch.empty(m, dtype=torch.int32, device=dev)
+    far_count = torch.empty(1, dtype=torch.int32, device=dev)
+    dist = torch.empty(m, dtype=torch.float32, device=dev)
+    idx = torch.empty(m, dtype=torch.int32, device=dev)
+    call("nksr_metric_nearest", svh.view(), xs, tn, ranges, box, n, query, qn, m, C.addressof(origin_host), START_LEVEL,
+         dist, idx, dot if both else None, far_list, far_count, stream_ptr(dev))
+    return dist, perm[idx.long()], dot
+
+
+def summarise(completeness: torch.Tensor, completeness_dot: torch.Tensor, accuracy: torch.Tensor,
+              accuracy_dot: torch.Tensor, thresholds=THRESHOLDS) -> dict:
+    """Every metric of the evaluator from the two distance and normal-agreement arrays, in fp64 (SPEC S18)."""
+    c, a = completeness.double(), accuracy.double()
+    th = torch.tensor(thresholds, dtype=torch.float64, device=c.device)
+    recall = (c[None, :] <= th[:, None]).double().mean(dim=1)
+    precision = (a[None, :] <= th[:, None]).double().mean(dim=1)
+    stats = torch.stack([c.mean(), (c * c).mean(), completeness_dot.double().mean(), a.mean(), (a * a).mean(),
+                         accuracy_dot.double().mean()])
+    comp, comp2, comp_n, acc, acc2, acc_n = stats.tolist()         # the one host read
+    p, r = precision.tolist(), recall.tolist()
+    fs = [2.0 * p[i] * r[i] / (p[i] + r[i]) if p[i] + r[i] > 0 else _NAN for i in range(len(p))]
+    return {
+        "completeness": comp, "accuracy": acc,
+        "normals completeness": comp_n, "normals accuracy": acc_n, "normals": 0.5 * comp_n + 0.5 * acc_n,
+        "completeness2": comp2, "accuracy2": acc2, "chamfer-L2": 0.5 * (comp2 + acc2),
+        "chamfer-L1": 0.5 * (comp + acc),
+        "f-precision": p[0], "f-recall": r[0], "f-score": fs[0], "f-score-15": fs[1], "f-score-20": fs[2],
+        "f-precision-outdoor": p[4], "f-recall-outdoor": r[4], "f-score-outdoor": fs[4],
+    }
+
+
+METRIC_KEYS = ("completeness", "accuracy", "normals completeness", "normals accuracy", "normals", "completeness2",
+               "accuracy2", "chamfer-L2", "chamfer-L1", "f-precision", "f-recall", "f-score", "f-score-15",
+               "f-score-20", "f-precision-outdoor", "f-recall-outdoor", "f-score-outdoor")
+
+
+def mesh_arrays(mesh):
+    """(v, f) of a DualMesh (.v, .f), a (v, f) pair or an object with `vertices` / `triangles` (an open3d mesh)."""
+    if isinstance(mesh, (tuple, list)) and len(mesh) == 2:
+        return mesh[0], mesh[1]
+    if hasattr(mesh, "v") and hasattr(mesh, "f"):
+        return mesh.v, mesh.f
+    if hasattr(mesh, "vertices") and hasattr(mesh, "triangles"):
+        return mesh.vertices, mesh.triangles
+    raise TypeError("mesh must be a DualMesh, a (v, f) pair or have `vertices` and `triangles`")
+
+
+class MeshEvaluator:
+    """Drop-in for the reference's metrics.MeshEvaluator: same constructor, class attributes, methods, keys and
+    definitions; CUDA only.  `o3d-iou` (a mesh-occupancy IoU on ray queries the reference takes from a package
+    outside its tree) is not provided."""
+
+    ESSENTIAL_METRICS = ["chamfer-L1", "f-score", "normals"]
+    ALL_METRICS = ["completeness", "accuracy", "normals completeness", "normals accuracy", "normals",
+                   "completeness2", "accuracy2", "chamfer-L2",
+                   "chamfer-L1", "f-precision", "f-recall", "f-score", "f-score-15", "f-score-20"]
+
+    def __init__(self, n_points=100000, metric_names=ALL_METRICS, device=None, seed: int = 0):
+        names = list(metric_names)
+        if "o3d-iou" in names:
+            raise ValueError("'o3d-iou' is not provided: it needs a ray-distance occupancy query of the mesh that the "
+                             "reference takes from a package outside its tree")
+        unknown = [k for k in names if k not in METRIC_KEYS]
+        if unknown:
+            raise ValueError(f"unknown metric names {unknown}; known: {list(METRIC_KEYS)}")
+        self.n_points = int(n_points)
+        self.thresholds = np.array(THRESHOLDS)
+        self.fidx = [0, 1, 2, 3, 4]
+        self.metric_names = names
+        self.device = torch.device(device) if device is not None else None
+        self.seed = int(seed)
+
+    def _device_for(self, a) -> torch.device:
+        if self.device is not None:
+            return self.device
+        if isinstance(a, torch.Tensor) and a.is_cuda:
+            return a.device
+        return torch.device("cuda", 0)
+
+    def eval_mesh(self, mesh, pointcloud_tgt, normals_tgt, onet_samples=None):
+        """Samples n_points on the mesh (area-uniform, triangle normals) and evaluates them against the target."""
+        v, f = mesh_arrays(mesh)
+        dev = self._device_for(v)
+        v = _as_tensor(v, dev, torch.float32).reshape(-1, 3)
+        f = _as_tensor(f, dev, torch.int32).reshape(-1, 3)
+        xyz, nrm, _ = sample_surface(v, f, self.n_points, self.seed)
+        return self._evaluate(xyz, pointcloud_tgt, nrm, normals_tgt, onet_samples, mesh)
+
+    def _evaluate(self, pointcloud, pointcloud_tgt, normals=None, normals_tgt=None, onet_samples=None, mesh=None):
+        dev = self._device_for(pointcloud)
+        if int(pointcloud.shape[0]) == 0:
+            _log.warning("Empty pointcloud / mesh detected! Return NaN metric!")
+            return {k: _NAN for k in self.metric_names}
+        pts = _as_tensor(pointcloud, dev, torch.float32).reshape(-1, 3)
+        tgt = _as_tensor(pointcloud_tgt, dev, torch.float32).reshape(-1, 3)
+        if tgt.shape[0] == 0:
+            raise NksrError("the target point cloud is empty")
+        nrm = _as_tensor(normals, dev, torch.float32).reshape(-1, 3) if normals is not None else None
+        nrm_t = _as_tensor(normals_tgt, dev, torch.float32).reshape(-1, 3) if normals_tgt is not None else None
+        comp, _, comp_dot = nearest_neighbours(tgt, pts, nrm_t, nrm)
+        acc, _, acc_dot = nearest_neighbours(pts, tgt, nrm, nrm_t)
+        out = summarise(comp, comp_dot, acc, acc_dot, tuple(self.thresholds.tolist()))
+        return {k: out[k] for k in self.metric_names}
+
+
+__all__ = ["MeshEvaluator", "sample_surface", "nearest_neighbours", "summarise", "mesh_arrays", "THRESHOLDS"]

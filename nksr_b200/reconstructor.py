@@ -65,11 +65,14 @@ def voxel_size_from_detail(xyz: torch.Tensor, detail_level: float) -> float:
 KNN_LEVELS = 7        # levels of the voxel hash behind the kNN search (cell size doubles per level)
 
 
-def _knn_hash(xyz: torch.Tensor, levels: int = KNN_LEVELS):
+def _knn_hash(xyz: torch.Tensor, levels: int = KNN_LEVELS, origin: Optional[torch.Tensor] = None):
     """Multi-level voxel hash of a cloud for neighbour searches: returns (perm, svh, base, ranges, origin) with the points
     Morton-sorted by `perm`, the hierarchy of their containing voxels (finest cell ~ a sixth of the mean point
     spacing, doubling per level), base[l][i] = containing voxel of sorted point i, ranges[offset_l + v] = [first,
-    last) sorted point of voxel v.  Keys are taken on coordinates shifted to the bounding-box corner."""
+    last) sorted point of voxel v.  Keys are taken on coordinates shifted to the bounding-box corner, or to `origin`
+    (a point at or below that corner, e.g. the corner of the cloud and its queries together) where given; an origin
+    further than 2^18 finest cells below the corner is raised to that distance, so that the cloud stays in the key
+    range."""
     dev, st = xyz.device, stream_ptr(xyz.device)
     n = xyz.shape[0]
     lo = xyz.min(dim=0).values
@@ -78,6 +81,8 @@ def _knn_hash(xyz: torch.Tensor, levels: int = KNN_LEVELS):
     dims = [max(e, 1e-3 * emax) for e in ext]
     h0 = 0.15 * (dims[0] * dims[1] * dims[2] / max(n, 1)) ** (1.0 / 3.0)
     h0 = float(torch.tensor(max(h0, emax / 2.0 ** 17), dtype=torch.float32).item())
+    if origin is not None:
+        lo = torch.maximum(torch.minimum(origin.to(lo), lo), lo - 2.0 ** 18 * h0)
     shifted = (xyz - lo).contiguous()
     hk = torch.empty(n, dtype=torch.int64, device=dev)
     status = torch.zeros(1, dtype=torch.int32, device=dev)
