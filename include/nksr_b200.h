@@ -288,6 +288,30 @@ NKSR_API int nksr_spmv_stream_planned(const int64_t* rowptr, const int32_t* col,
                              float* y, int64_t n, int64_t nnz, int64_t split_row, int64_t split_nnz,
                              void* plan_buf, void* stream);
 
+/* -- the inference system without the matrix (csrc/operator.cu): A x = E^T W E x + w_reg R x applied straight from the
+ * kernel rows, which are read once per application.  c: e_pos / range_pos of the sorted positions, e_nrm / range_nrm /
+ * t_nrm of the sorted normal locations, nrm_compact 0 (gradient rows, nksr_build_rows mode 1) or 1 (compact lines, mode
+ * 2); mblocks and split_level are ignored.  base_pos / base_nrm: [depth][m] containing voxel per level of the same
+ * sorted locations (nksr_locate).  The workspace holds 2 x 27 planes of n floats of per-(stencil slot, voxel) partial
+ * sums. */
+NKSR_API size_t nksr_op_workspace_bytes(const nksr_svh_t* svh);
+/* once per system: rhs b = E^T W t and the Jacobi diagonal diag(A); also clears the workspace for nksr_op_apply */
+NKSR_API int nksr_op_setup(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
+                           const int32_t* base_pos, const int32_t* base_nrm, float* rhs, float* diag, void* ws,
+                           size_t ws_bytes, void* stream);
+/* y = A x over a workspace that nksr_op_setup prepared for the same hierarchy, features and constraints.  No atomics:
+ * the same x gives bitwise the same y */
+NKSR_API int nksr_op_apply(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
+                           const int32_t* base_pos, const int32_t* base_nrm, const float* x, float* y, void* ws,
+                           size_t ws_bytes, void* stream);
+/* nksr_pcg_solve with the matrix-free A: op_ws prepared by nksr_op_setup (which gave diag and b), ws of
+ * nksr_pcg_workspace_bytes(n) bytes.  profile != 0: info[2] / info[3] time every application of A */
+NKSR_API int nksr_pcg_solve_matrix_free(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
+                                        const int32_t* base_pos, const int32_t* base_nrm, const float* diag,
+                                        const float* b, float* x, float tol, int max_iter, int check_every,
+                                        int profile, void* op_ws, size_t op_ws_bytes, void* ws, size_t ws_bytes,
+                                        double* info, void* stream);
+
 /* ---- e: step kernels of the multi-GPU solve (one global system, SURVEY section 8e mapping B).  A
  * Chronopoulos-Gear arrangement of the same Jacobi-PCG: per iteration ONE halo exchange of u = M^-1 r, one
  * SpMV on the owned rows and ONE fused all-reduce of red[3] = {(r,u), (w,u), (r,r)}; the caller issues the

@@ -17,6 +17,7 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "operator.cuh"
 #include "spmv_stream.cuh"
 
 namespace {
@@ -242,14 +243,30 @@ static PcgWs carve(void* ws, int64_t n) {
   return w;
 }
 
+// The operator A of a PCG: an assembled CSR matrix (row kernel, or the tile stream when `plan` is set) or, when `mf` is
+// set, the matrix-free E^T W E + w_reg R of csrc/operator.cu.  Either way one application writes Ap and the p.Ap
+// partials of kGrid blocks; the vector kernels, the graph replay and the verdict do not depend on which.
+struct PcgOperator {
+  const int64_t* rowptr;
+  const int32_t* col;
+  const float* val;
+  const SpmvPlan* plan;
+  const MfOperator* mf;
+};
+
 // one PCG iteration on stream s (rz buffers alternate with the iteration parity)
-static void launch_iteration(const int64_t* rowptr, const int32_t* col, const float* val, const float* diag, float* x,
-                             int64_t n, const PcgWs& w, int parity, cudaStream_t s, cudaEvent_t e0, cudaEvent_t e1,
-                             const SpmvPlan* plan) {
+static void launch_iteration(const PcgOperator& A, const float* diag, float* x, int64_t n, const PcgWs& w, int parity,
+                             cudaStream_t s, cudaEvent_t e0, cudaEvent_t e1) {
+  const int64_t* rowptr = A.rowptr;
+  const int32_t* col = A.col;
+  const float* val = A.val;
+  const SpmvPlan* plan = A.plan;
   double* rz_cur = parity ? w.rz1 : w.rz0;
   double* rz_new = parity ? w.rz0 : w.rz1;
   if (e0) cudaEventRecord(e0, s);
-  if (plan) {   // tile stream through the TMA engine + boundary rows, long coarse rows warp per row, then p.Ap
+  if (A.mf) {
+    mf_apply_launch(*A.mf, w.p, w.ap, w.pap, kGrid, &w.ctrl->done, s);
+  } else if (plan) {   // tile stream through the TMA engine + boundary rows, long coarse rows warp per row, then p.Ap
     spmv_stream_launch(rowptr, col, val, w.p, w.ap, *plan, &w.ctrl->done, s);
     if (plan->n_rows < n)
       k_spmv<false><<<kGrid, kBlock, 0, s>>>(rowptr + plan->n_rows, col, val, w.p, w.ap + plan->n_rows,
@@ -291,9 +308,9 @@ size_t nksr_pcg_workspace_bytes(int64_t n) {
 
 }  // extern "C"
 
-static int pcg_solve_impl(const int64_t* rowptr, const int32_t* col, const float* val, const float* diag,
-                          const float* b, float* x, int64_t n, float tol, int max_iter, int check_every, int profile,
-                          void* ws, size_t ws_bytes, double* info, void* stream, const SpmvPlan* plan) {
+static int pcg_solve_impl(const PcgOperator& A, const float* diag, const float* b, float* x, int64_t n, float tol,
+                          int max_iter, int check_every, int profile, void* ws, size_t ws_bytes, double* info,
+                          void* stream) {
   if (n <= 0 || !info || max_iter < 0) return NKSR_E_INVALID;
   if (ws_bytes < nksr_pcg_workspace_bytes(n)) return NKSR_E_WORKSPACE;
   if (check_every < 1) check_every = 1;
@@ -310,7 +327,7 @@ static int pcg_solve_impl(const int64_t* rowptr, const int32_t* col, const float
   PcgCtrl host;
   int rc = NKSR_OK;
   if (profile) {
-    // CUDA events around every SpMV launch on this stream (info[2], info[3]); plain launches, checked
+    // CUDA events around every application of A on this stream (info[2], info[3]); plain launches, checked
     // every `check_every` iterations like the graph path
     const int kMaxEv = 512;
     cudaEvent_t ev[2 * kMaxEv];
@@ -320,8 +337,8 @@ static int pcg_solve_impl(const int64_t* rowptr, const int32_t* col, const float
     while (rc == NKSR_OK && launched < max_iter) {
       for (int j = 0; j < check_every && launched < max_iter; ++j, ++launched) {
         const bool timed = n_ev < kMaxEv;
-        launch_iteration(rowptr, col, val, diag, x, n, w, launched & 1, s, timed ? ev[2 * n_ev] : nullptr,
-                         timed ? ev[2 * n_ev + 1] : nullptr, plan);
+        launch_iteration(A, diag, x, n, w, launched & 1, s, timed ? ev[2 * n_ev] : nullptr,
+                         timed ? ev[2 * n_ev + 1] : nullptr);
         if (timed) ++n_ev;
       }
       rc = read_ctrl(w.ctrl, &host, s);
@@ -352,7 +369,7 @@ static int pcg_solve_impl(const int64_t* rowptr, const int32_t* col, const float
       ok = cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
       if (ok) {
         for (int j = 0; j < per_graph; ++j)
-          launch_iteration(rowptr, col, val, diag, x, n, w, j & 1, cap, nullptr, nullptr, plan);
+          launch_iteration(A, diag, x, n, w, j & 1, cap, nullptr, nullptr);
         ok = cudaStreamEndCapture(cap, &graph) == cudaSuccess && graph != nullptr;
       }
       if (ok) ok = cudaGraphInstantiate(&exec, graph, 0) == cudaSuccess;
@@ -384,8 +401,19 @@ extern "C" {
 int nksr_pcg_solve(const int64_t* rowptr, const int32_t* col, const float* val, const float* diag, const float* b,
                    float* x, int64_t n, float tol, int max_iter, int check_every, int profile, void* ws,
                    size_t ws_bytes, double* info, void* stream) {
-  return pcg_solve_impl(rowptr, col, val, diag, b, x, n, tol, max_iter, check_every, profile, ws, ws_bytes, info,
-                        stream, nullptr);
+  const PcgOperator A{rowptr, col, val, nullptr, nullptr};
+  return pcg_solve_impl(A, diag, b, x, n, tol, max_iter, check_every, profile, ws, ws_bytes, info, stream);
+}
+
+int nksr_pcg_solve_matrix_free(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
+                               const int32_t* base_pos, const int32_t* base_nrm, const float* diag, const float* b,
+                               float* x, float tol, int max_iter, int check_every, int profile, void* op_ws,
+                               size_t op_ws_bytes, void* ws, size_t ws_bytes, double* info, void* stream) {
+  MfOperator mf;
+  const int rc = mf_operator_make(svh, feat, c, base_pos, base_nrm, op_ws, op_ws_bytes, &mf);
+  if (rc != NKSR_OK) return rc;
+  const PcgOperator A{nullptr, nullptr, nullptr, nullptr, &mf};
+  return pcg_solve_impl(A, diag, b, x, mf.n, tol, max_iter, check_every, profile, ws, ws_bytes, info, stream);
 }
 
 size_t nksr_pcg_stream_workspace_bytes(int64_t n, int64_t nnz) {
@@ -403,12 +431,12 @@ int nksr_pcg_solve_stream(const int64_t* rowptr, const int32_t* col, const float
   if (cudaMemsetAsync(plan.stats, 0, 4 * sizeof(unsigned long long), as_stream(stream)) != cudaSuccess)
     return NKSR_E_CUDA;
   if (split_row == 0 || split_nnz == 0)     // nothing to stream: the plain solver
-    return pcg_solve_impl(rowptr, col, val, diag, b, x, n, tol, max_iter, check_every, profile, ws, base, info, stream,
-                          nullptr);
+    return pcg_solve_impl(PcgOperator{rowptr, col, val, nullptr, nullptr}, diag, b, x, n, tol, max_iter, check_every,
+                          profile, ws, base, info, stream);
   if (spmv_stream_prepare() != NKSR_OK || spmv_stream_sm_count() <= 0) return NKSR_E_CUDA;
   if (spmv_plan_build(rowptr, plan, as_stream(stream)) != NKSR_OK) return NKSR_E_CUDA;
-  return pcg_solve_impl(rowptr, col, val, diag, b, x, n, tol, max_iter, check_every, profile, ws, base, info, stream,
-                        &plan);
+  return pcg_solve_impl(PcgOperator{rowptr, col, val, &plan, nullptr}, diag, b, x, n, tol, max_iter, check_every,
+                        profile, ws, base, info, stream);
 }
 
 size_t nksr_spmv_plan_bytes(int64_t nnz) { return spmv_plan_bytes(nnz > 0 ? nnz : 1); }

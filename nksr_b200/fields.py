@@ -33,6 +33,10 @@ DEFAULT_FILL = "brick"
 # 'brick' bricks a fine level only when it holds at least this many constraint locations per voxel (measured on H100:
 # faster than the row fill at 18 per voxel, slower at 1.7, 4.9 and 8.2; DESIGN 4.1)
 BRICK_MIN_LOCATIONS_PER_VOXEL = 12.0
+# the matrix-free operator is the default (with approx_kernel_grad) from this many unknowns on.  Measured on H100: 15 %
+# faster per bench.py step at 17.1 M unknowns (cfg4), 11 % slower at 2.0 M (cfg3, whose solve takes 16 iterations of an
+# operator that costs 2.5 packed SpMVs); the crossover between the two was not measured (DESIGN 4.2.1)
+MATRIX_FREE_MIN_UNKNOWNS = 8_000_000
 
 
 _TOTAL_MEMORY = {}
@@ -43,6 +47,18 @@ def _total_memory(dev) -> int:
     if key not in _TOTAL_MEMORY:
         _TOTAL_MEMORY[key] = int(torch.cuda.get_device_properties(dev).total_memory * 0.94)   # driver / context reserve
     return _TOTAL_MEMORY[key]
+
+
+def operator_bytes_per_apply(svh, n_pos: int, n_nrm: int, nrm_lines: int, channels: int) -> int:
+    """Byte model of one matrix-free application of A (csrc/operator.cu), from shapes: the kernel rows (128 B per
+    location, level and line: nrm_lines = 1 compact, 3 full), the locations' containing voxels (4 B per level), nbr27
+    read once per voxel by each kernel, the planar partial sums written and gathered once (27 floats per voxel each),
+    the features z (4 C B per voxel) and x read twice and y written (12 B per voxel).  Voxels without locations are
+    counted as if they had some, so it is an upper bound of the algorithmic bytes.  bench.py's roofline_spmv
+    (8 nnz + 12 n) describes the assembled matrix, not this path."""
+    L, n = svh.depth, svh.num_unknowns
+    rows = 128 * L * (n_pos + nrm_lines * n_nrm)
+    return int(rows + 4 * L * (n_pos + n_nrm) + 2 * 108 * n + 2 * 108 * n + 4 * channels * n + 12 * n)
 
 
 class EvaluationResult(SimpleNamespace):
@@ -235,11 +251,104 @@ class KernelField(BaseField):
             self.alpha = _KernelSolve.apply(self, (pos_xyz, normal_xyz, pos_weight, normal_weight, reg_weight), nv,
                                             *self.z)
             return self
+        if self._operator() == "matrix_free" and not self.solver_config.get("keep_system"):
+            self.alpha = self._solve_matrix_free(pos_xyz, normal_xyz, normal_value, pos_weight, normal_weight,
+                                                 reg_weight)
+            return self
         sysm = self.assemble(pos_xyz, normal_xyz, normal_value, pos_weight, normal_weight, reg_weight)
         self.alpha = self._pcg(sysm, sysm.rhs)
         if self.solver_config.get("keep_system"):
             self.system = sysm
         return self
+
+    def _operator(self):
+        """solver_config['operator'] or NKSR_OPERATOR: 'matrix_free' (A applied from the kernel rows, csrc/operator.cu)
+        or 'assembled' (the CSR Gram matrix).  Default: matrix-free with approx_kernel_grad (compact rows) on systems of
+        at least MATRIX_FREE_MIN_UNKNOWNS unknowns, assembled otherwise.  A Gram fill chosen explicitly
+        (solver_config['fill'] or NKSR_FILL) asks for the matrix that fill builds, so it too selects the assembled
+        operator unless the operator is given as well.  Grad-recording solves, keep_system and the global solve always
+        assemble."""
+        op = self.solver_config.get("operator") or os.environ.get("NKSR_OPERATOR")
+        if op is None:
+            big = self.svh.num_unknowns >= MATRIX_FREE_MIN_UNKNOWNS
+            fill_chosen = bool(self.solver_config.get("fill") or os.environ.get("NKSR_FILL"))
+            op = "matrix_free" if self.approx_kernel_grad and big and not fill_chosen else "assembled"
+        if op not in ("matrix_free", "assembled"):
+            raise ValueError("solver_config['operator'] must be 'matrix_free' or 'assembled'")
+        return op
+
+    def _solve_matrix_free(self, pos_xyz, normal_xyz, normal_value, pos_weight, normal_weight, reg_weight):
+        """Jacobi-PCG on A = E^T W E + reg R without assembling A (DESIGN 4.2.1): kernel rows (compact gradient lines
+        with approx_kernel_grad), then rhs and diagonal (nksr_op_setup), then the PCG, whose every iteration applies A
+        from the rows (nksr_pcg_solve_matrix_free).  No count, placement, blocks or fill; solve_info['nnz'] = 0."""
+        op = self.matrix_free_system(pos_xyz, normal_xyz, normal_value, pos_weight, normal_weight, reg_weight)
+        svh, dev, n = self.svh, self.svh.device, op.n
+        alpha = torch.empty(n, dtype=torch.float32, device=dev)
+        info = (C.c_double * 8)()
+        profile = int(bool(self.solver_config.get("profile")))
+        nb = call("nksr_pcg_workspace_bytes", n)
+        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+        call("nksr_pcg_solve_matrix_free", svh.view(), self.feat_view(), op.cs, op.base_pos, op.base_nrm, op.diag,
+             op.rhs, alpha, float(self.solver_config["tol"]), int(self.solver_config["max_iter"]),
+             int(self.solver_config["check_every"]), profile, op.ws, op.ws_bytes, ws, nb, info, stream_ptr(dev))
+        tm = getattr(self, "_timer", None) or _lib.StageTimer(dev, enabled=False)
+        tm.mark("pcg")
+        self._pcg_report(info, n, 0, False, operator="matrix_free", operator_bytes_per_apply=op.bytes_per_apply)
+        return alpha
+
+    def matrix_free_system(self, pos_xyz, normal_xyz=None, normal_value=None, pos_weight=1.0, normal_weight=1.0,
+                           reg_weight=1.0):
+        """Kernel rows of the sorted constraint locations and the operator's setup (nksr_op_setup): returns
+        .rhs, .diag, .n and what apply_operator needs (the rows, the constraint struct, the operator's workspace)."""
+        svh = self.svh
+        dev = svh.device
+        _lib.require_cuda(pos_xyz, "pos_xyz")
+        st = stream_ptr(dev)
+        n = svh.num_unknowns
+        if n == 0:
+            raise _lib.NksrError("empty hierarchy: nothing to solve")
+        if n >= 2 ** 31:
+            raise _lib.NksrError("more than 2^31 unknowns: shard the cloud (chunk_size)")
+        pos_xyz = pos_xyz.detach().to(dev, torch.float32).contiguous()
+        cs = _lib.ConstraintsT()
+        loc_pos = self._sorted_locations(pos_xyz)
+        _, _, base_pos, range_pos, e_pos = self._sorted_rows(pos_xyz, 0, loc=loc_pos)
+        cs.e_pos, cs.range_pos, cs.n_pos, cs.w_pos = e_pos.data_ptr(), range_pos.data_ptr(), pos_xyz.shape[0], float(pos_weight)
+        keep = [e_pos, range_pos]
+        base_nrm, lines, K = None, 0, 0
+        if normal_xyz is not None and normal_xyz.shape[0] > 0:
+            normal_xyz = normal_xyz.detach().to(dev, torch.float32).contiguous()
+            normal_value = normal_value.detach().to(dev, torch.float32).contiguous()
+            mode = 2 if self.approx_kernel_grad else 1          # compact lines: one 128 B line per location and level
+            loc_nrm = self._sorted_locations(normal_xyz, normal_value)
+            _, t_nrm, base_nrm, range_nrm, e_nrm = self._sorted_rows(normal_xyz, mode, normal_value, loc=loc_nrm)
+            keep += [t_nrm, range_nrm, e_nrm]
+            cs.e_nrm, cs.range_nrm, cs.t_nrm = e_nrm.data_ptr(), range_nrm.data_ptr(), t_nrm.data_ptr()
+            K, lines = normal_xyz.shape[0], (1 if mode == 2 else 3)
+            cs.n_nrm, cs.w_nrm, cs.nrm_compact = K, float(normal_weight), int(mode == 2)
+        else:
+            cs.e_nrm = cs.range_nrm = cs.t_nrm = None
+            cs.n_nrm, cs.w_nrm, cs.nrm_compact = 0, 0.0, 0
+        cs.w_reg = float(reg_weight)
+        cs.mblocks, cs.split_level = None, svh.depth
+        tm = getattr(self, "_timer", None) or _lib.StageTimer(dev, enabled=False)
+        tm.mark("kernel_rows")
+        nb_op = call("nksr_op_workspace_bytes", svh.view())
+        op_ws = torch.empty(nb_op, dtype=torch.uint8, device=dev)
+        rhs = torch.empty(n, dtype=torch.float32, device=dev)
+        diag = torch.empty(n, dtype=torch.float32, device=dev)
+        call("nksr_op_setup", svh.view(), self.feat_view(), cs, base_pos, base_nrm, rhs, diag, op_ws, nb_op, st)
+        tm.mark("operator_setup")
+        return SimpleNamespace(cs=cs, base_pos=base_pos, base_nrm=base_nrm, rhs=rhs, diag=diag, ws=op_ws,
+                               ws_bytes=nb_op, n=n, keep=keep,
+                               bytes_per_apply=operator_bytes_per_apply(svh, pos_xyz.shape[0], K, lines, self.channels))
+
+    def apply_operator(self, op, x: torch.Tensor) -> torch.Tensor:
+        """y = A x for a system of matrix_free_system (nksr_op_apply)"""
+        y = torch.empty(op.n, dtype=torch.float32, device=self.svh.device)
+        call("nksr_op_apply", self.svh.view(), self.feat_view(), op.cs, op.base_pos, op.base_nrm,
+             x.to(torch.float32).contiguous(), y, op.ws, op.ws_bytes, stream_ptr(self.svh.device))
+        return y
 
     def _pcg(self, sysm, rhs, adjoint: bool = False):
         """Jacobi-PCG on the assembled system: the forward solve (A alpha = b) and the adjoint solve of the backward
@@ -275,15 +384,22 @@ class KernelField(BaseField):
                  float(self.solver_config["tol"]), int(self.solver_config["max_iter"]),
                  int(self.solver_config["check_every"]), profile, ws, nb, info, stream_ptr(dev))
         tm.mark("adjoint_pcg" if adjoint else "pcg")
+        extra = {"operator": "assembled"}
+        if packed is not None:
+            extra.update(spmv_packed_tiles=packed[0], spmv_packed_entries=packed[1], spmv_streamed_tiles=packed[2],
+                         spmv_streamed_entries=packed[3])
+        self._pcg_report(info, n, sysm.nnz, adjoint, **extra)
+        return alpha
+
+    def _pcg_report(self, info, n, nnz, adjoint, **extra):
+        """solve_info from a PCG's info[] (the forward replaces it, the adjoint adds to it); a breakdown raises,
+        max_iter warns"""
         status = int(info[4])                       # 0 converged, 1 max_iter reached, 2 NaN / breakdown
         if adjoint:
             self.solve_info.update(adjoint_iterations=int(info[0]), adjoint_relative_residual=float(info[1]))
         else:
             self.solve_info = {"iterations": int(info[0]), "relative_residual": float(info[1]), "n": n,
-                               "nnz": sysm.nnz, "converged": status == 0}
-            if packed is not None:
-                self.solve_info.update(spmv_packed_tiles=packed[0], spmv_packed_entries=packed[1],
-                                       spmv_streamed_tiles=packed[2], spmv_streamed_entries=packed[3])
+                               "nnz": nnz, "converged": status == 0, **extra}
         what = "adjoint PCG" if adjoint else "PCG"
         if status == 2:
             raise _lib.NksrError(f"{what} broke down (non-finite residual) after {int(info[0])} iterations: the system "
@@ -291,11 +407,10 @@ class KernelField(BaseField):
         if status == 1 and int(self.solver_config["max_iter"]) > 0:
             warnings.warn(f"nksr_b200 {what} stopped at max_iter={int(self.solver_config['max_iter'])} with relative "
                           f"residual {float(info[1]):.3e} > tol={float(self.solver_config['tol']):.1e}", RuntimeWarning)
-        if profile and not adjoint:
+        if self.solver_config.get("profile") and not adjoint:
             self.solve_info.update(spmv_ms=float(info[2]), spmv_launches=int(info[3]))
         if self.solver_config.get("verbose"):
-            print(f"[nksr_b200] {what}: n={n} nnz={sysm.nnz} iters={int(info[0])} relres={float(info[1]):.3e}")
-        return alpha
+            print(f"[nksr_b200] {what}: n={n} nnz={nnz} iters={int(info[0])} relres={float(info[1]):.3e}")
 
     def _count_and_place(self, n, keep):
         """structure-only part of the assembly (row lengths, placement tables, row pointers): depends on the hierarchy
