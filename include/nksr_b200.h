@@ -289,21 +289,31 @@ NKSR_API int nksr_spmv_stream_planned(const int64_t* rowptr, const int32_t* col,
                              void* plan_buf, void* stream);
 
 /* -- the inference system without the matrix (csrc/operator.cu): A x = E^T W E x + w_reg R x applied straight from the
- * kernel rows, which are read once per application.  c: e_pos / range_pos of the sorted positions, e_nrm / range_nrm /
- * t_nrm of the sorted normal locations, nrm_compact 0 (gradient rows, nksr_build_rows mode 1) or 1 (compact lines, mode
- * 2); mblocks and split_level are ignored.  base_pos / base_nrm: [depth][m] containing voxel per level of the same
- * sorted locations (nksr_locate).  The workspace holds 2 x 27 planes of n floats of per-(stencil slot, voxel) partial
- * sums. */
-NKSR_API size_t nksr_op_workspace_bytes(const nksr_svh_t* svh);
-/* once per system: rhs b = E^T W t and the Jacobi diagonal diag(A); also clears the workspace for nksr_op_apply */
+ * kernel rows, which are read once per application.  c: e_pos of the sorted positions, e_nrm / t_nrm of the sorted
+ * normal locations, nrm_compact 0 (gradient rows, nksr_build_rows mode 1) or 1 (compact lines, mode 2); range_pos,
+ * range_nrm, mblocks and split_level are ignored.  base_pos / base_nrm: [depth][m] containing voxel per level of the
+ * same sorted locations (nksr_locate); key_pos / key_nrm: their half-voxel keys (nksr_point_half_keys), ascending.
+ * The workspace holds 2 x 27 planes of n floats of per-(stencil slot, voxel) partial sums, the merged location order
+ * with its containing voxels (4 (depth + 1) bytes per location), and the work items of at most item_size locations
+ * with their edge partials; nksr_op_workspace_bytes gives its size for c->n_pos + c->n_nrm locations. */
+NKSR_API size_t nksr_op_workspace_bytes(const nksr_svh_t* svh, const nksr_constraints_t* c, int item_size);
+/* once per system: merges the two location orders, cuts the work items (item_size >= 1: at most that many locations,
+ * cut only between voxels of levels <= 2, never across a top-level voxel; one such voxel with more locations is an
+ * item of its own), then rhs b = E^T W t and the Jacobi diagonal diag(A) */
 NKSR_API int nksr_op_setup(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
-                           const int32_t* base_pos, const int32_t* base_nrm, float* rhs, float* diag, void* ws,
-                           size_t ws_bytes, void* stream);
+                           const int32_t* base_pos, const int32_t* base_nrm, const int64_t* key_pos,
+                           const int64_t* key_nrm, int item_size, float* rhs, float* diag, void* ws, size_t ws_bytes,
+                           void* stream);
 /* y = A x over a workspace that nksr_op_setup prepared for the same hierarchy, features and constraints.  No atomics:
  * the same x gives bitwise the same y */
 NKSR_API int nksr_op_apply(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
                            const int32_t* base_pos, const int32_t* base_nrm, const float* x, float* y, void* ws,
                            size_t ws_bytes, void* stream);
+/* out[4] (host) = byte offsets in a workspace of ws_bytes bytes of the merged location order ([m] int32: r >= 0 position
+ * r, ~r normal location r), its containing voxels ([depth][m] int32), the item count (int32) and the items ([count]
+ * int4: begin, end, flags 1 first / 2 last item of its top-level voxel, 0) */
+NKSR_API int nksr_op_workspace_layout(const nksr_svh_t* svh, const nksr_constraints_t* c, size_t ws_bytes,
+                                      int64_t* out);
 /* nksr_pcg_solve with the matrix-free A: op_ws prepared by nksr_op_setup (which gave diag and b), ws of
  * nksr_pcg_workspace_bytes(n) bytes.  profile != 0: info[2] / info[3] time every application of A */
 NKSR_API int nksr_pcg_solve_matrix_free(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,

@@ -96,9 +96,10 @@ _SIGNATURES = {
     "nksr_spmv_plan_build": ("i", "p" + "qqqq" + "pzp"),
     "nksr_spmv_plan_stats": ("i", "ppp"),
     "nksr_spmv_stream_planned": ("i", "ppppp" + "qqqq" + "pp"),
-    "nksr_op_workspace_bytes": ("z", "S"),
-    "nksr_op_setup": ("i", "SFK" + "pppppzp"),
+    "nksr_op_workspace_bytes": ("z", "SKi"),
+    "nksr_op_setup": ("i", "SFK" + "ppppi" + "pppzp"),
     "nksr_op_apply": ("i", "SFK" + "pppppzp"),
+    "nksr_op_workspace_layout": ("i", "SKzp"),
     "nksr_pcg_solve_matrix_free": ("i", "SFK" + "ppppp" + "fiii" + "pzpzdp"),
     "nksr_dcg_workspace_bytes": ("z", ""),
     "nksr_dcg_init": ("i", "pppppppp" + "q" + "pz" + "pp"),

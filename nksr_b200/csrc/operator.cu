@@ -1,168 +1,406 @@
 // Matrix-free application of the inference system A = E^T W E + w_reg R (SPEC S5) straight from the kernel rows, for the
 // PCG of KernelField.solve: no count, placement, blocks or fill, and no CSR matrix.  DESIGN 4.2.1.
 //
-// k_op_gather_scatter: one warp per top-level voxel, lane = stencil slot.  The warp walks the voxel's contiguous range of
-// Morton-sorted position locations, then of normal locations.  Per location r it loads the r's lines of every level
-// once, forms t_r = w_r E_r x (three values for a gradient location, one per axis) from the x values of the containing
-// voxel's 27 neighbours -- fetched once per run of locations with the same containing voxel u_l -- and adds E_l[r][s] t_r
-// into a register accumulator per level.  When u_l changes, the accumulator goes to the planar partial sums P[s][u]
-// (27 planes of n floats).  A level-l voxel's locations are contiguous and lie inside one top voxel's range, so one warp
-// owns every P[.][u] it writes: positions store, normals then add, in a fixed order -- no atomics, and the result is
-// bitwise repeatable.  Voxels without locations are never written, and stay zero from the setup's clear.
+// Setup (nksr_op_setup, once per solve) merges the Morton-sorted positions and normal locations into one sequence by
+// their half-voxel keys (positions first on equal keys), so that every voxel's locations of both kinds are one
+// contiguous run at every level.  It cuts each top-level voxel's run into work items of at most S locations, cut only
+// where no voxel of a level <= kCutLevel continues (a single such voxel longer than S is an item of its own).
+//
+// k_op_walk: a persistent grid of warps steps over the items, lane = stencil slot.  Per location r the warp loads r's
+// lines of every level once, forms t_r = w_r E_r x (three values for a gradient location, one per axis) from the x
+// values of the containing voxel's 27 neighbours -- fetched once per run of locations with the same containing voxel
+// u_l, the next locations' nbr27 rows and x values requested under the current one's reductions -- and adds
+// E_l[r][s] t_r into a register accumulator per level.  When u_l changes, the accumulator is stored once to the planar
+// partial sums P[s][u] (27 planes of n floats).  A voxel of a level <= kCutLevel lies inside one item; a coarser voxel's
+// run may span items, and then every item stores its piece to an edge buffer, which k_op_edges sums in item order and
+// stores to P once.  No atomics: each P[.][u] has one writer, and the result is bitwise repeatable and independent of
+// the grid.  Voxels without locations are never written, and stay zero from the setup's clear.
 //
 // k_op_apply: one thread per unknown, levels concatenated, grid-stride.  y_i = sum_s P[s][nbr27(i)[26 - s]] (u's slot s
 // is i exactly when i's slot 26 - s is u) + w_reg sum_s B3(d_s) <z_i, z_n> x_n over the 27 neighbours n = nbr27(i)[s]:
 // the regulariser of gram_row_regulariser, formed on the fly.
 //
-// Setup (once per solve): the same two kernels with t_r = w_r * target (the right-hand side) and w_r E^2 (the Jacobi
-// diagonal) accumulated into a second set of planes.
+// Setup also runs the walk with t_r = w_r * target (the right-hand side) and w_r E^2 (the Jacobi diagonal) accumulated
+// into a second set of planes.
+#include <cub/cub.cuh>
+
 #include "gram_common.cuh"
 #include "operator.cuh"
 
 namespace {
 
-constexpr int kOpWarps = 8;
+constexpr int kOpWarps = 4;          // warps per block of the walk
 constexpr int kApplyBlock = 256;
+constexpr int kEdgeBlock = 256;
+// items are cut at boundaries of the voxels of levels <= kCutLevel; the nbr27 rows / x values of levels below
+// kPrefetchLevels are requested two / one locations ahead (0: on demand, as each new containing voxel starts).  The
+// macros exist to measure the alternatives (DESIGN 4.2.1); the defaults are what the measurements chose.
+#ifndef NKSR_OP_CUT_LEVEL
+#define NKSR_OP_CUT_LEVEL 2
+#endif
+#ifndef NKSR_OP_PREFETCH_LEVELS
+#define NKSR_OP_PREFETCH_LEVELS 2
+#endif
+constexpr int kCutLevel = NKSR_OP_CUT_LEVEL;
+constexpr int kPrefetchLevels = NKSR_OP_PREFETCH_LEVELS;
+constexpr int kItemFirst = 1, kItemLast = 2;   // item flags: first / last item of its top voxel
 
 // row forms: value rows (positions), compact gradient lines (approx_kernel_grad), three full gradient rows
 enum { kValue = 0, kCompact = 1, kFull = 2 };
 
-template <int KIND, int MAXL, bool SETUP>
-__device__ __forceinline__ void op_walk(const nksr_svh_t& svh, const float* __restrict__ e,
-                                        const int32_t* __restrict__ base, const float* __restrict__ tgt, int64_t m,
-                                        float w, int b, int end, const float* __restrict__ x, float* __restrict__ P,
-                                        float* __restrict__ Pd, const int32_t* __restrict__ add_if, int64_t n,
-                                        int lane) {
-  constexpr int LINES = KIND == kFull ? 3 : 1;   // 128-byte lines per (location, level)
-  constexpr int AX = KIND == kValue ? 1 : 3;     // rows per (location, level)
+__device__ __forceinline__ int op_cut_level(int depth) { return depth - 1 < kCutLevel ? depth - 1 : kCutLevel; }
+
+// the edge partials of the rhs / application (e) and of the diagonal (d), after the items, each 256-byte aligned; laid
+// out for the capacity nksr_op_setup recorded, whatever workspace size a later application is given
+struct EdgeBuffers { float* e; float* d; };
+__device__ __forceinline__ EdgeBuffers op_edge_buffers(const MfOperator& op) {
+  const uint64_t mi = (uint64_t)*op.max_items;
+  const uint64_t a = (reinterpret_cast<uint64_t>(op.items) + mi * sizeof(int4) + 255) & ~(uint64_t)255;
+  const uint64_t b = (a + mi * op.edge_levels * 2 * 27 * sizeof(float) + 255) & ~(uint64_t)255;
+  return {reinterpret_cast<float*>(a), reinterpret_cast<float*>(b)};
+}
+
+// ------------------------------------------------------------------------------------------------- setup: the items
+// merged position of every location: positions first on equal keys (a stable merge of the two sorted key lists)
+__global__ void k_op_merge(const int64_t* __restrict__ kp, int64_t np, const int64_t* __restrict__ kn, int64_t nn,
+                           const int32_t* __restrict__ bp, const int32_t* __restrict__ bn, int L,
+                           int32_t* __restrict__ seq, int32_t* __restrict__ vox) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int64_t m = np + nn;
+  if (i >= m) return;
+  const bool pos = i < np;
+  const int64_t r = pos ? i : i - np;
+  const int64_t key = pos ? kp[r] : kn[r];
+  const int64_t* other = pos ? kn : kp;
+  int64_t lo = 0, hi = pos ? nn : np;   // positions: #normals with key < k; normals: #positions with key <= k
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    const int64_t v = __ldg(other + mid);
+    if (pos ? v < key : v <= key) lo = mid + 1; else hi = mid;
+  }
+  const int64_t rank = r + lo;
+  seq[rank] = pos ? (int32_t)r : ~(int32_t)r;
+  const int32_t* b = pos ? bp : bn;
+  const int64_t nb = pos ? np : nn;
+  for (int l = 0; l < L; ++l) vox[l * m + rank] = __ldg(b + l * nb + r);
+}
+
+// merged range of every top-level voxel (zero-length for voxels without locations: the workspace starts cleared)
+__global__ void k_op_top_ranges(const int32_t* __restrict__ vt, int64_t m, int2* __restrict__ top) {
+  const int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (k >= m) return;
+  const int t = vt[k];
+  if (t < 0) return;
+  if (k == 0 || vt[k - 1] != t) top[t].x = (int)k;
+  if (k == m - 1 || vt[k + 1] != t) top[t].y = (int)(k + 1);
+}
+
+// one warp per top voxel: greedy items of at most S locations, cut only before a location k where no voxel of a level
+// <= cut continues from k - 1; when there is no such k within S locations, the item runs to the next one.
+// !WRITE: cnt[g] = items of voxel g.  WRITE: items at ofs[g], and the last voxel's warp stores the item count.
+template <bool WRITE>
+__global__ void k_op_cut(const int32_t* __restrict__ vox, int64_t m, const int2* __restrict__ top, int64_t n_top,
+                         int cut, int S, int32_t* __restrict__ cnt, const int32_t* __restrict__ ofs,
+                         int4* __restrict__ items, int32_t* __restrict__ n_items) {
+  const int lane = threadIdx.x & 31;
+  const int64_t g = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+  if (g >= n_top) return;
+  const int2 rg = top[g];
+  const int s = rg.x, e = rg.y;
+  auto legal = [&](int k) {
+    for (int l = 0; l <= cut; ++l) {
+      const int p = __ldg(vox + l * m + k - 1);
+      if (p >= 0 && p == __ldg(vox + l * m + k)) return false;
+    }
+    return true;
+  };
+  const int o = WRITE ? ofs[g] : 0;
+  int a = s, c = 0;
+  while (a < e) {
+    const int64_t lim = (int64_t)a + S < e ? (int64_t)a + S : e;
+    int b = -1;
+    if (lim == e) {
+      b = e;
+    } else {
+      for (int hi = (int)lim; hi > a && b < 0; hi -= 32) {   // the largest legal cut in (a, lim]
+        const int k = hi - lane;
+        const unsigned bal = __ballot_sync(0xffffffffu, k > a && legal(k));
+        if (bal) b = hi - (__ffs(bal) - 1);
+      }
+      for (int lo = (int)lim + 1; b < 0; lo += 32) {          // none: the first one after lim (e at the latest)
+        const int k = lo + lane;
+        const unsigned bal = __ballot_sync(0xffffffffu, k >= e || legal(k));
+        if (bal) b = lo + __ffs(bal) - 1;
+      }
+    }
+    if (WRITE && lane == 0) items[o + c] = make_int4(a, b, (a == s ? kItemFirst : 0) | (b == e ? kItemLast : 0), 0);
+    ++c;
+    a = b;
+  }
+  if (!WRITE && lane == 0) cnt[g] = c;
+  if (WRITE && lane == 0 && g == n_top - 1) *n_items = o + c;
+}
+
+// ------------------------------------------------------------------------------------------- the walk of one item
+template <int NKIND, int MAXL, bool SETUP>
+__device__ __forceinline__ void op_walk_item(const MfOperator& op, const float* __restrict__ x, int it, int4 item,
+                                             EdgeBuffers eb, int lane) {
+  constexpr int LINES = NKIND == kFull ? 3 : 1;     // 128-byte lines per (location, level) of the widest row
+  constexpr int PF = MAXL < kPrefetchLevels ? MAXL : kPrefetchLevels;
+  const nksr_svh_t& svh = op.svh;
   const int L = svh.depth;
-  int cur[MAXL];
-  float acc[MAXL], accd[MAXL], xc[MAXL];
-#pragma unroll
-  for (int l = 0; l < MAXL; ++l) { cur[l] = -1; acc[l] = 0.f; accd[l] = 0.f; xc[l] = 0.f; }
+  const int cut = op_cut_level(L);
+  const int64_t m = op.m;
+  const int32_t* __restrict__ vox = op.vox;
+  const int b = item.x, e = item.y;
   const int sl = lane < 27 ? lane : 13;
   const CompactSpline spline(c_d27[sl][0], c_d27[sl][1], c_d27[sl][2]);
   const float inv_w0 = 1.f / svh.voxel_size;
 
-  // P[s][u] (+)= acc: lanes < 27; `add_if` (the normal pass): add when the position pass wrote the voxel
-  auto flush = [&](int l) {
-    const int u = cur[l];
-    if (lane < 27) {
-      const int64_t g = svh.offset[l] + u;
-      const bool add = add_if != nullptr && __ldg(add_if + 2 * g) < __ldg(add_if + 2 * g + 1);
-      const int64_t q = (int64_t)lane * n + g;
-      P[q] = add ? P[q] + acc[l] : acc[l];
-      if (SETUP) Pd[q] = add ? Pd[q] + accd[l] : accd[l];
-    }
-    acc[l] = 0.f;
-    accd[l] = 0.f;
+  // the voxels just before (lane l) and after (lane 16 + l) the item on level l, inside its top voxel
+  int edge_nb = -1;
+  if (lane < L && !(item.z & kItemFirst)) edge_nb = __ldg(vox + lane * m + b - 1);
+  else if (lane >= 16 && lane - 16 < L && !(item.z & kItemLast)) edge_nb = __ldg(vox + (lane - 16) * m + e);
+
+  // two windows of 32 merged locations: sequence entry and containing voxels, lane j = location k0 + j (+ 32)
+  int wq, wq2, wv[MAXL], wv2[MAXL];
+  auto load_win = [&](int k0, int& q, int (&v)[MAXL]) {
+    const int k = k0 + lane;
+    const bool in = k < e;
+    q = in ? __ldg(op.seq + k) : 0;
+#pragma unroll
+    for (int l = 0; l < MAXL; ++l) v[l] = (in && l < L) ? __ldg(vox + l * m + k) : -1;
   };
+  auto win = [&](int d, int v, int v2) {   // d = k - k0 in [0, 64), warp-uniform
+    return d < 32 ? __shfl_sync(0xffffffffu, v, d) : __shfl_sync(0xffffffffu, v2, d - 32);
+  };
+  int k0 = b;
+  load_win(b, wq, wv);
+  load_win(b + 32, wq2, wv2);
 
   float nx[MAXL][LINES];   // the next location's lines, requested one location ahead
-  auto load_lines = [&](int r, float (&dst)[MAXL][LINES]) {
-    const float* p = e + (int64_t)r * L * LINES * NKSR_ROW_STRIDE + lane;
+  auto load_lines = [&](int q, float (&dst)[MAXL][LINES]) {
+    if (q >= 0) {
+      const float* p = op.cs.e_pos + (int64_t)q * L * NKSR_ROW_STRIDE + lane;
 #pragma unroll
-    for (int l = 0; l < MAXL; ++l)
+      for (int l = 0; l < MAXL; ++l)
 #pragma unroll
-      for (int a = 0; a < LINES; ++a)
-        dst[l][a] = l < L ? __ldcs(p + (l * LINES + a) * NKSR_ROW_STRIDE) : 0.f;
-  };
-  load_lines(b, nx);
-  int bl[MAXL];            // containing voxels of 32 consecutive locations, lane j = location r0 + j
-  for (int r = b; r < end; ++r) {
-    const int j = (r - b) & 31;
-    if (j == 0) {
+        for (int a = 0; a < LINES; ++a) dst[l][a] = (a == 0 && l < L) ? __ldcs(p + l * NKSR_ROW_STRIDE) : 0.f;
+    } else {
+      const float* p = op.cs.e_nrm + (int64_t)~q * L * LINES * NKSR_ROW_STRIDE + lane;
 #pragma unroll
-      for (int l = 0; l < MAXL; ++l) bl[l] = (l < L && r + lane < end) ? __ldg(base + (int64_t)l * m + r + lane) : -1;
+      for (int l = 0; l < MAXL; ++l)
+#pragma unroll
+        for (int a = 0; a < LINES; ++a) dst[l][a] = l < L ? __ldcs(p + (l * LINES + a) * NKSR_ROW_STRIDE) : 0.f;
     }
+  };
+
+  int cur[MAXL];
+  float acc[MAXL], accd[MAXL], xc[MAXL];
+#pragma unroll
+  for (int l = 0; l < MAXL; ++l) { cur[l] = -1; acc[l] = 0.f; accd[l] = 0.f; xc[l] = 0.f; }
+  unsigned first = 0xffffffffu;   // bit l: the current level-l run started at the item's first location
+
+  // P[s][u] = acc, or the item's edge slot when u's run continues into the previous or the next item
+  auto flush = [&](int l, bool last) {
+    const int u = cur[l];
+    bool to_edge = false;
+    int side = 0;
+    if (l > cut) {
+      const int pv = __shfl_sync(0xffffffffu, edge_nb, l), nv = __shfl_sync(0xffffffffu, edge_nb, 16 + l);
+      const bool f = (first >> l) & 1u;
+      to_edge = (f && pv == u) || (last && nv == u);
+      side = f ? 0 : 1;
+    }
+    if (lane < 27) {
+      if (to_edge) {
+        const int64_t q = (((int64_t)it * op.edge_levels + (l - cut - 1)) * 2 + side) * 27 + lane;
+        eb.e[q] = acc[l];
+        if (SETUP) eb.d[q] = accd[l];
+      } else {
+        const int64_t q = (int64_t)lane * op.n + svh.offset[l] + u;
+        op.P[q] = acc[l];
+        if (SETUP) op.Pd[q] = accd[l];
+      }
+    }
+  };
+
+  // pipelined levels: vk = v_l(k), vk1 = v_l(k + 1); xq = x at vk's stencil (requested when vk starts a run),
+  // nq = vk1's nbr27 entry (requested when vk1 starts a run)
+  constexpr int PFA = PF > 0 ? PF : 1;
+  int vk[PFA], vk1[PFA], nq[PFA];
+  float xq[PFA];
+#pragma unroll
+  for (int l = 0; l < PF; ++l) {
+    vk[l] = l < L ? win(0, wv[l], wv2[l]) : -1;
+    vk1[l] = (l < L && b + 1 < e) ? win(1, wv[l], wv2[l]) : -1;
+    xq[l] = 0.f;
+    nq[l] = -1;
+    if (!SETUP) {
+      const int nb = (vk[l] >= 0 && lane < 27) ? __ldg(svh.nbr27[l] + (int64_t)vk[l] * 27 + lane) : -1;
+      xq[l] = nb >= 0 ? __ldg(x + svh.offset[l] + nb) : 0.f;
+      nq[l] = (vk1[l] != vk[l] && vk1[l] >= 0 && lane < 27) ? __ldg(svh.nbr27[l] + (int64_t)vk1[l] * 27 + lane) : -1;
+    }
+  }
+  int q = win(0, wq, wq2);
+  load_lines(q, nx);
+
+  for (int k = b; k < e; ++k) {
     float ln[MAXL][LINES];
 #pragma unroll
     for (int l = 0; l < MAXL; ++l)
 #pragma unroll
       for (int a = 0; a < LINES; ++a) ln[l][a] = nx[l][a];
-    if (r + 1 < end) load_lines(r + 1, nx);
+    const int qn = k + 1 < e ? win(k + 1 - k0, wq, wq2) : 0;
+    if (k + 1 < e) load_lines(qn, nx);
+
+    // a new containing voxel: the finished run goes out, the new one's x values come in
 #pragma unroll
     for (int l = 0; l < MAXL; ++l) {
       if (l < L) {
-        const int u = __shfl_sync(0xffffffffu, bl[l], j);
-        if (u != cur[l]) {
-          if (cur[l] >= 0) flush(l);
-          cur[l] = u;
+        const int v = l < PF ? vk[l < PF ? l : 0] : win(k - k0, wv[l], wv2[l]);
+        if (v != cur[l]) {
+          if (cur[l] >= 0) flush(l, false);
+          if (k > b) first &= ~(1u << l);
+          cur[l] = v;
+          acc[l] = 0.f;
+          accd[l] = 0.f;
           if (!SETUP) {
-            const int nb = (u >= 0 && lane < 27) ? __ldg(svh.nbr27[l] + (int64_t)u * 27 + lane) : -1;
-            xc[l] = nb >= 0 ? __ldg(x + svh.offset[l] + nb) : 0.f;
+            if (l < PF) {
+              xc[l] = xq[l < PF ? l : 0];
+            } else {
+              const int nb = (v >= 0 && lane < 27) ? __ldg(svh.nbr27[l] + (int64_t)v * 27 + lane) : -1;
+              xc[l] = nb >= 0 ? __ldg(x + svh.offset[l] + nb) : 0.f;
+            }
           }
         }
       }
     }
-    // this lane's entries of the location's rows (zero on a level without containing voxel, and in lanes >= 27)
-    float ev[MAXL][AX];
+    // requested under this location's reductions: x for location k + 1, nbr27 for location k + 2
 #pragma unroll
-    for (int l = 0; l < MAXL; ++l) {
-      if (KIND == kCompact) {
-        float e0 = 0.f, e1 = 0.f, e2 = 0.f;
-        if (l < L) spline.grad_rows(ln[l][0], inv_w0 * __int_as_float((127 - l) << 23), lane, e0, e1, e2);
-        ev[l][0] = e0;
-        ev[l][AX > 1 ? 1 : 0] = e1;
-        ev[l][AX > 2 ? 2 : 0] = e2;
+    for (int l = 0; l < PF; ++l) {
+      if (l < L) {
+        const int v2 = k + 2 < e ? win(k + 2 - k0, wv[l], wv2[l]) : -1;
+        if (!SETUP) {
+          xq[l] = (vk1[l] != vk[l] && nq[l] >= 0) ? __ldg(x + svh.offset[l] + nq[l]) : 0.f;
+          nq[l] = (v2 != vk1[l] && v2 >= 0 && lane < 27) ? __ldg(svh.nbr27[l] + (int64_t)v2 * 27 + lane) : -1;
+        }
+        vk[l] = vk1[l];
+        vk1[l] = v2;
+      }
+    }
+
+    // this location's rows: t = w E x, then acc += E t
+    auto visit = [&](auto kind_tag) {
+      constexpr int KIND = decltype(kind_tag)::value;
+      constexpr int AX = KIND == kValue ? 1 : 3;
+      const float w = KIND == kValue ? op.cs.w_pos : op.cs.w_nrm;
+      float ev[MAXL][AX];   // zero on a level without containing voxel, and in lanes >= 27
+#pragma unroll
+      for (int l = 0; l < MAXL; ++l) {
+        if (KIND == kCompact) {
+          float e0 = 0.f, e1 = 0.f, e2 = 0.f;
+          if (l < L) spline.grad_rows(ln[l][0], inv_w0 * __int_as_float((127 - l) << 23), lane, e0, e1, e2);
+          ev[l][0] = e0;
+          ev[l][AX > 1 ? 1 : 0] = e1;
+          ev[l][AX > 2 ? 2 : 0] = e2;
+        } else {
+#pragma unroll
+          for (int a = 0; a < AX; ++a) ev[l][a] = ln[l][a];
+        }
+      }
+      float t[AX];
+      if (SETUP) {
+#pragma unroll
+        for (int a = 0; a < AX; ++a) t[a] = KIND == kValue ? 0.f : w * __ldg(op.cs.t_nrm + (int64_t)~q * 3 + a);
       } else {
 #pragma unroll
-        for (int a = 0; a < AX; ++a) ev[l][a] = ln[l][a];
-      }
-    }
-    float t[AX];
-    if (SETUP) {
+        for (int a = 0; a < AX; ++a) {
+          float s = 0.f;
 #pragma unroll
-      for (int a = 0; a < AX; ++a) t[a] = KIND == kValue ? 0.f : w * __ldg(tgt + (int64_t)r * 3 + a);
-    } else {
+          for (int l = 0; l < MAXL; ++l) s = fmaf(ev[l][a], xc[l], s);
+          t[a] = s;
+        }
 #pragma unroll
-      for (int a = 0; a < AX; ++a) {
-        float s = 0.f;
-#pragma unroll
-        for (int l = 0; l < MAXL; ++l) s = fmaf(ev[l][a], xc[l], s);
-        t[a] = s;
+        for (int a = 0; a < AX; ++a) t[a] = w * warp_sum(t[a]);
       }
 #pragma unroll
-      for (int a = 0; a < AX; ++a) t[a] = w * warp_sum(t[a]);
-    }
+      for (int l = 0; l < MAXL; ++l) {
 #pragma unroll
-    for (int l = 0; l < MAXL; ++l) {
-#pragma unroll
-      for (int a = 0; a < AX; ++a) {
-        acc[l] = fmaf(ev[l][a], t[a], acc[l]);
-        if (SETUP) accd[l] = fmaf(w * ev[l][a], ev[l][a], accd[l]);
+        for (int a = 0; a < AX; ++a) {
+          acc[l] = fmaf(ev[l][a], t[a], acc[l]);
+          if (SETUP) accd[l] = fmaf(w * ev[l][a], ev[l][a], accd[l]);
+        }
       }
+    };
+    if (q >= 0) visit(std::integral_constant<int, kValue>());
+    else visit(std::integral_constant<int, NKIND>());
+
+    q = qn;
+    if (k + 1 - k0 == 32) {   // slide the windows
+      k0 += 32;
+      wq = wq2;
+#pragma unroll
+      for (int l = 0; l < MAXL; ++l) wv[l] = wv2[l];
+      load_win(k0 + 32, wq2, wv2);
     }
   }
 #pragma unroll
   for (int l = 0; l < MAXL; ++l)
-    if (l < L && cur[l] >= 0) flush(l);
+    if (l < L && cur[l] >= 0) flush(l, true);
 }
 
 template <int NKIND, int MAXL, bool SETUP>
-__global__ void __launch_bounds__(kOpWarps * 32)
-k_op_gather_scatter(nksr_svh_t svh, nksr_constraints_t cs, const int32_t* __restrict__ base_pos,
-                    const int32_t* __restrict__ base_nrm, const float* __restrict__ x, float* __restrict__ P,
-                    float* __restrict__ Pd, int64_t n, const int* __restrict__ done) {
+__global__ void __launch_bounds__(kOpWarps * 32, MAXL <= 4 ? 5 : 1)   // depth <= 4: at most 102 registers
+k_op_walk(MfOperator op, const float* __restrict__ x, const int* __restrict__ done) {
   if (done && *done) return;
   const int lane = threadIdx.x & 31;
-  const int64_t top = blockIdx.x * (int64_t)kOpWarps + (threadIdx.x >> 5);
-  const int T = svh.depth - 1;
-  if (top >= svh.n[T]) return;
-  const int64_t g = svh.offset[T] + top;
-  int pb = 0, pe = 0;
-  if (cs.n_pos > 0) {
-    pb = __ldg(cs.range_pos + 2 * g);
-    pe = __ldg(cs.range_pos + 2 * g + 1);
-    if (pb < pe)
-      op_walk<kValue, MAXL, SETUP>(svh, cs.e_pos, base_pos, nullptr, cs.n_pos, cs.w_pos, pb, pe, x, P, Pd, nullptr, n,
-                                   lane);
-  }
-  if (cs.n_nrm > 0) {
-    const int nb = __ldg(cs.range_nrm + 2 * g), ne = __ldg(cs.range_nrm + 2 * g + 1);
-    if (nb < ne)
-      op_walk<NKIND, MAXL, SETUP>(svh, cs.e_nrm, base_nrm, cs.t_nrm, cs.n_nrm, cs.w_nrm, nb, ne, x, P, Pd,
-                                  pb < pe ? cs.range_pos : nullptr, n, lane);
+  const int n_items = *op.n_items;
+  const EdgeBuffers eb = op_edge_buffers(op);
+  for (int it = blockIdx.x * kOpWarps + (threadIdx.x >> 5); it < n_items; it += gridDim.x * kOpWarps)
+    op_walk_item<NKIND, MAXL, SETUP>(op, x, it, op.items[it], eb, lane);
+}
+
+// one warp per (item, level above the cut): a run that starts in the item and continues into the next ones is summed
+// over its pieces in item order and stored to P once
+template <bool SETUP>
+__global__ void __launch_bounds__(kEdgeBlock) k_op_edges(MfOperator op, const int* __restrict__ done) {
+  if (done && *done) return;
+  const int NL = op.edge_levels;
+  const int lane = threadIdx.x & 31;
+  const int cut = op_cut_level(op.svh.depth);
+  const int64_t units = (int64_t)*op.n_items * NL;
+  const EdgeBuffers eb = op_edge_buffers(op);
+  const int64_t stride = (int64_t)gridDim.x * (kEdgeBlock / 32);
+  for (int64_t w = (blockIdx.x * (int64_t)kEdgeBlock + threadIdx.x) >> 5; w < units; w += stride) {
+    const int it = (int)(w / NL), j = (int)(w % NL), l = cut + 1 + j;
+    const int4 item = op.items[it];
+    if (item.z & kItemLast) continue;
+    const int32_t* v = op.vox + l * op.m;
+    const int u = __ldg(v + item.y - 1);
+    if (u < 0 || __ldg(v + item.y) != u) continue;                            // the item's last run ends in it
+    const bool in_first = __ldg(v + item.x) == u;
+    if (in_first && !(item.z & kItemFirst) && __ldg(v + item.x - 1) == u) continue;   // summed where it starts
+    int64_t q = (((int64_t)it * NL + j) * 2 + (in_first ? 0 : 1)) * 27 + lane;
+    float s = 0.f, sd = 0.f;
+    if (lane < 27) {
+      s = eb.e[q];
+      if (SETUP) sd = eb.d[q];
+    }
+    for (int i = it + 1;; ++i) {
+      const int4 nxt = op.items[i];
+      q = (((int64_t)i * NL + j) * 2) * 27 + lane;
+      if (lane < 27) {
+        s += eb.e[q];
+        if (SETUP) sd += eb.d[q];
+      }
+      if ((nxt.z & kItemLast) || __ldg(v + nxt.y) != u) break;
+    }
+    if (lane < 27) {
+      const int64_t p = (int64_t)lane * op.n + op.svh.offset[l] + u;
+      op.P[p] = s;
+      if (SETUP) op.Pd[p] = sd;
+    }
   }
 }
 
@@ -227,26 +465,81 @@ k_op_apply(nksr_svh_t svh, nksr_feat_t feat, float w_reg, const float* __restric
   }
 }
 
+// -------------------------------------------------------------------------------------------------------- host side
 size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
 int64_t op_unknowns(const nksr_svh_t& svh) { return svh.offset[svh.depth - 1] + svh.n[svh.depth - 1]; }
 
+int edge_levels(const nksr_svh_t& svh) {
+  const int cut = svh.depth - 1 < kCutLevel ? svh.depth - 1 : kCutLevel;
+  return svh.depth - 1 - cut;
+}
+
+// workspace: P, Pd, the merged sequence and its voxels, top ranges, item counts and offsets, the item count, the scan's
+// scratch (the fixed part), then as many items with their edge slots as the rest holds
+struct OpLayout {
+  size_t P, Pd, seq, vox, top, cnt, ofs, n_items, max_items, scan, scan_bytes, fixed;
+  size_t per_item;   // item record + its edge slots (rhs and diagonal)
+};
+
+OpLayout op_layout(const nksr_svh_t& svh, int64_t m) {
+  OpLayout o;
+  const int64_t n = op_unknowns(svh), n_top = svh.n[svh.depth - 1];
+  o.scan_bytes = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, o.scan_bytes, (const int32_t*)nullptr, (int32_t*)nullptr,
+                                (int)(n_top > 0 ? n_top : 1));
+  size_t at = 0;
+  auto take = [&](size_t bytes) { const size_t p = at; at += align256(bytes); return p; };
+  o.P = take((size_t)27 * n * sizeof(float));
+  o.Pd = take((size_t)27 * n * sizeof(float));
+  o.seq = take((size_t)m * sizeof(int32_t));
+  o.vox = take((size_t)svh.depth * m * sizeof(int32_t));
+  o.top = take((size_t)n_top * sizeof(int2));
+  o.cnt = take((size_t)n_top * sizeof(int32_t));
+  o.ofs = take((size_t)n_top * sizeof(int32_t));
+  o.n_items = take(sizeof(int32_t));
+  o.max_items = take(sizeof(int64_t));
+  o.scan = take(o.scan_bytes);
+  o.fixed = at;
+  o.per_item = sizeof(int4) + 2 * (size_t)edge_levels(svh) * 2 * 27 * sizeof(float);
+  return o;
+}
+
+// greedy items: two consecutive items of one top voxel hold more than S locations together
+int64_t op_max_items(const nksr_svh_t& svh, int64_t m, int S) {
+  return 2 * ((m + S - 1) / S) + svh.n[svh.depth - 1];
+}
+
+int sm_count() {
+  int dev = 0, sms = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    return 132;
+  return sms > 0 ? sms : 132;
+}
+
 template <bool SETUP>
-int gather_scatter_launch(const MfOperator& op, const float* x, const int* done, cudaStream_t s) {
-  const int64_t n_top = op.svh.n[op.svh.depth - 1];
-  if (n_top == 0) return NKSR_OK;
-  const int grid = (int)((n_top + kOpWarps - 1) / kOpWarps);
+void walk_launch(const MfOperator& op, const float* x, const int* done, cudaStream_t s) {
   const bool compact = op.cs.nrm_compact == 1;
-#define NKSR_GS(NK, ML) \
-  k_op_gather_scatter<NK, ML, SETUP><<<grid, kOpWarps * 32, 0, s>>>(op.svh, op.cs, op.base_pos, op.base_nrm, x, op.P, \
-                                                                     op.Pd, op.n, done)
+#define NKSR_WALK(NK, ML) k_op_walk<NK, ML, SETUP><<<op.walk_grid, kOpWarps * 32, 0, s>>>(op, x, done)
   if (op.svh.depth <= 4) {
-    if (compact) NKSR_GS(kCompact, 4); else NKSR_GS(kFull, 4);
+    if (compact) NKSR_WALK(kCompact, 4); else NKSR_WALK(kFull, 4);
   } else {
-    if (compact) NKSR_GS(kCompact, NKSR_MAX_DEPTH); else NKSR_GS(kFull, NKSR_MAX_DEPTH);
+    if (compact) NKSR_WALK(kCompact, NKSR_MAX_DEPTH); else NKSR_WALK(kFull, NKSR_MAX_DEPTH);
   }
-#undef NKSR_GS
-  return NKSR_OK;
+#undef NKSR_WALK
+  if (op.edge_levels > 0) k_op_edges<SETUP><<<op.edge_grid, kEdgeBlock, 0, s>>>(op, done);
+}
+
+// resident blocks per SM of the walk kernel this operator launches
+int walk_blocks_per_sm(const MfOperator& op) {
+  const bool compact = op.cs.nrm_compact == 1, deep = op.svh.depth > 4;
+  const void* f = deep ? (compact ? (const void*)k_op_walk<kCompact, NKSR_MAX_DEPTH, false>
+                                  : (const void*)k_op_walk<kFull, NKSR_MAX_DEPTH, false>)
+                       : (compact ? (const void*)k_op_walk<kCompact, 4, false> : (const void*)k_op_walk<kFull, 4, false>);
+  int blocks = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, f, kOpWarps * 32, 0) != cudaSuccess || blocks < 1)
+    blocks = 1;
+  return blocks;
 }
 
 bool op_valid(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c, const int32_t* base_pos,
@@ -254,9 +547,9 @@ bool op_valid(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constra
   if (!svh || !feat || !c || svh->depth < 1 || svh->depth > NKSR_MAX_DEPTH) return false;
   if (feat->channels < 1 || feat->channels > 32) return false;
   if (c->nrm_compact != 0 && c->nrm_compact != 1) return false;
-  if (c->n_pos < 0 || c->n_nrm < 0 || c->n_pos >= INT32_MAX || c->n_nrm >= INT32_MAX) return false;
-  if (c->n_pos > 0 && (!c->e_pos || !c->range_pos || !base_pos)) return false;
-  if (c->n_nrm > 0 && (!c->e_nrm || !c->range_nrm || !c->t_nrm || !base_nrm)) return false;
+  if (c->n_pos < 0 || c->n_nrm < 0 || c->n_pos + c->n_nrm >= INT32_MAX) return false;
+  if (c->n_pos > 0 && (!c->e_pos || !base_pos)) return false;
+  if (c->n_nrm > 0 && (!c->e_nrm || !c->t_nrm || !base_nrm)) return false;
   for (int l = 0; l < svh->depth; ++l)
     if (svh->n[l] > 0 && (!svh->nbr27[l] || !feat->z[l])) return false;
   return op_unknowns(*svh) > 0;
@@ -271,9 +564,31 @@ MfOperator make_op(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_co
   op.base_pos = base_pos;
   op.base_nrm = base_nrm;
   op.n = op_unknowns(*svh);
-  op.P = reinterpret_cast<float*>(ws);
-  op.Pd = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(ws) + align256((size_t)27 * op.n * sizeof(float)));
+  op.m = c->n_pos + c->n_nrm;
+  const OpLayout o = op_layout(*svh, op.m);
+  unsigned char* w = reinterpret_cast<unsigned char*>(ws);
+  op.P = reinterpret_cast<float*>(w + o.P);
+  op.Pd = reinterpret_cast<float*>(w + o.Pd);
+  op.seq = reinterpret_cast<int32_t*>(w + o.seq);
+  op.vox = reinterpret_cast<int32_t*>(w + o.vox);
+  op.top = reinterpret_cast<int2*>(w + o.top);
+  op.cnt = reinterpret_cast<int32_t*>(w + o.cnt);
+  op.ofs = reinterpret_cast<int32_t*>(w + o.ofs);
+  op.n_items = reinterpret_cast<int32_t*>(w + o.n_items);
+  op.scan_tmp = w + o.scan;
+  op.scan_bytes = o.scan_bytes;
+  op.edge_levels = edge_levels(*svh);
+  op.max_items = reinterpret_cast<int64_t*>(w + o.max_items);
+  op.items = reinterpret_cast<int4*>(w + o.fixed);
+  const int sms = sm_count();
+  op.walk_grid = sms * walk_blocks_per_sm(op);
+  op.edge_grid = sms * 8;
   return op;
+}
+
+size_t workspace_bytes(const nksr_svh_t& svh, int64_t m, int item_size) {
+  const OpLayout o = op_layout(svh, m);
+  return o.fixed + (size_t)op_max_items(svh, m, item_size) * o.per_item + 768;
 }
 
 }  // namespace
@@ -281,14 +596,14 @@ MfOperator make_op(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_co
 int mf_operator_make(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
                      const int32_t* base_pos, const int32_t* base_nrm, void* ws, size_t ws_bytes, MfOperator* out) {
   if (!op_valid(svh, feat, c, base_pos, base_nrm) || !ws || !out) return NKSR_E_INVALID;
-  if (ws_bytes < nksr_op_workspace_bytes(svh)) return NKSR_E_WORKSPACE;
+  if (ws_bytes < op_layout(*svh, c->n_pos + c->n_nrm).fixed + 768) return NKSR_E_WORKSPACE;
   *out = make_op(svh, feat, c, base_pos, base_nrm, ws);
   return NKSR_OK;
 }
 
 int mf_apply_launch(const MfOperator& op, const float* x, float* y, double* pap, int blocks, const int* done,
                     cudaStream_t s) {
-  gather_scatter_launch<false>(op, x, done, s);
+  walk_launch<false>(op, x, done, s);
   k_op_apply<false><<<blocks, kApplyBlock, 0, s>>>(op.svh, op.feat, op.cs.w_reg, op.P, nullptr, x, y, nullptr, op.n,
                                                    pap, done);
   return NKSR_OK;
@@ -296,20 +611,44 @@ int mf_apply_launch(const MfOperator& op, const float* x, float* y, double* pap,
 
 extern "C" {
 
-size_t nksr_op_workspace_bytes(const nksr_svh_t* svh) {
-  if (!svh || svh->depth < 1 || svh->depth > NKSR_MAX_DEPTH) return 0;
-  return 2 * align256((size_t)27 * op_unknowns(*svh) * sizeof(float)) + 256;
+size_t nksr_op_workspace_bytes(const nksr_svh_t* svh, const nksr_constraints_t* c, int item_size) {
+  if (!svh || !c || svh->depth < 1 || svh->depth > NKSR_MAX_DEPTH || item_size < 1) return 0;
+  if (c->n_pos < 0 || c->n_nrm < 0) return 0;
+  return workspace_bytes(*svh, c->n_pos + c->n_nrm, item_size);
 }
 
 int nksr_op_setup(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c, const int32_t* base_pos,
-                  const int32_t* base_nrm, float* rhs, float* diag, void* ws, size_t ws_bytes, void* stream) {
-  if (!op_valid(svh, feat, c, base_pos, base_nrm) || !rhs || !diag || !ws) return NKSR_E_INVALID;
-  if (ws_bytes < nksr_op_workspace_bytes(svh)) return NKSR_E_WORKSPACE;
+                  const int32_t* base_nrm, const int64_t* key_pos, const int64_t* key_nrm, int item_size, float* rhs,
+                  float* diag, void* ws, size_t ws_bytes, void* stream) {
+  if (!op_valid(svh, feat, c, base_pos, base_nrm) || !rhs || !diag || !ws || item_size < 1) return NKSR_E_INVALID;
+  if ((c->n_pos > 0 && !key_pos) || (c->n_nrm > 0 && !key_nrm)) return NKSR_E_INVALID;
+  const int64_t m = c->n_pos + c->n_nrm;
+  if (ws_bytes < workspace_bytes(*svh, m, item_size)) return NKSR_E_WORKSPACE;
   cudaStream_t s = as_stream(stream);
   const MfOperator op = make_op(svh, feat, c, base_pos, base_nrm, ws);
-  // every plane starts at zero: the voxels without locations are never written, here or by nksr_op_apply
-  if (cudaMemsetAsync(ws, 0, nksr_op_workspace_bytes(svh), s) != cudaSuccess) return NKSR_E_CUDA;
-  gather_scatter_launch<true>(op, nullptr, nullptr, s);
+  // every plane starts at zero (the voxels without locations are never written, here or by nksr_op_apply), and so do
+  // the top ranges and the item count.  The tail holds as many items as fit; the kernels lay it out from the
+  // capacity recorded here, so later applications need not be given the same workspace size
+  const OpLayout o = op_layout(*svh, m);
+  const int64_t max_items = (int64_t)((ws_bytes - o.fixed - 768) / o.per_item);
+  if (cudaMemsetAsync(ws, 0, o.fixed, s) != cudaSuccess) return NKSR_E_CUDA;
+  if (cudaMemcpyAsync(op.max_items, &max_items, sizeof(int64_t), cudaMemcpyHostToDevice, s) != cudaSuccess)
+    return NKSR_E_CUDA;
+  const int64_t n_top = svh->n[svh->depth - 1];
+  if (m > 0 && n_top > 0) {
+    k_op_merge<<<grid_for(m, 256), 256, 0, s>>>(key_pos, c->n_pos, key_nrm, c->n_nrm, base_pos, base_nrm, svh->depth,
+                                               op.seq, op.vox);
+    k_op_top_ranges<<<grid_for(m, 256), 256, 0, s>>>(op.vox + (int64_t)(svh->depth - 1) * m, m, op.top);
+    const int cut = svh->depth - 1 < kCutLevel ? svh->depth - 1 : kCutLevel;
+    const int grid = grid_for(n_top * 32, 256);
+    k_op_cut<false><<<grid, 256, 0, s>>>(op.vox, m, op.top, n_top, cut, item_size, op.cnt, nullptr, nullptr, nullptr);
+    size_t tb = op.scan_bytes;
+    if (cub::DeviceScan::ExclusiveSum(op.scan_tmp, tb, op.cnt, op.ofs, (int)n_top, s) != cudaSuccess)
+      return NKSR_E_CUDA;
+    k_op_cut<true><<<grid, 256, 0, s>>>(op.vox, m, op.top, n_top, cut, item_size, nullptr, op.ofs, op.items,
+                                        op.n_items);
+    walk_launch<true>(op, nullptr, nullptr, s);
+  }
   const int grid = grid_for(op.n, kApplyBlock);
   k_op_apply<true><<<grid, kApplyBlock, 0, s>>>(op.svh, op.feat, op.cs.w_reg, op.P, op.Pd, nullptr, rhs, diag, op.n,
                                                 nullptr, nullptr);
@@ -320,10 +659,23 @@ int nksr_op_setup(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_con
 int nksr_op_apply(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c, const int32_t* base_pos,
                   const int32_t* base_nrm, const float* x, float* y, void* ws, size_t ws_bytes, void* stream) {
   if (!op_valid(svh, feat, c, base_pos, base_nrm) || !x || !y || !ws) return NKSR_E_INVALID;
-  if (ws_bytes < nksr_op_workspace_bytes(svh)) return NKSR_E_WORKSPACE;
-  const MfOperator op = make_op(svh, feat, c, base_pos, base_nrm, ws);
+  MfOperator op;
+  const int rc = mf_operator_make(svh, feat, c, base_pos, base_nrm, ws, ws_bytes, &op);
+  if (rc != NKSR_OK) return rc;
   mf_apply_launch(op, x, y, nullptr, grid_for(op.n, kApplyBlock), nullptr, as_stream(stream));
   NKSR_CHECK_LAUNCH();
+  return NKSR_OK;
+}
+
+int nksr_op_workspace_layout(const nksr_svh_t* svh, const nksr_constraints_t* c, size_t ws_bytes, int64_t* out) {
+  if (!svh || !c || !out || svh->depth < 1 || svh->depth > NKSR_MAX_DEPTH || c->n_pos < 0 || c->n_nrm < 0)
+    return NKSR_E_INVALID;
+  const OpLayout o = op_layout(*svh, c->n_pos + c->n_nrm);
+  if (ws_bytes < o.fixed + 768) return NKSR_E_WORKSPACE;
+  out[0] = (int64_t)o.seq;
+  out[1] = (int64_t)o.vox;
+  out[2] = (int64_t)o.n_items;
+  out[3] = (int64_t)o.fixed;
   return NKSR_OK;
 }
 

@@ -12,6 +12,22 @@ struct MfOperator {
   float* P;                  // [27][n]: per (stencil slot, voxel) partial sums of E^T W E x
   float* Pd;                 // [27][n]: the diagonal's partial sums (setup only)
   int64_t n;
+  // the merged walk (nksr_op_setup builds it): positions and normal locations in one half-voxel key order
+  int32_t* seq;              // [m] merged location: r >= 0 position r, ~r normal location r
+  int32_t* vox;              // [depth][m] containing voxel per level, merged order, -1 when inactive
+  int2* top;                 // [n_top] merged range of every top-level voxel
+  int32_t* cnt;              // [n_top] items per top voxel, then their exclusive scan in ofs
+  int32_t* ofs;
+  int32_t* n_items;          // device: number of work items
+  void* scan_tmp;
+  size_t scan_bytes;
+  int64_t* max_items;        // device: the item capacity nksr_op_setup laid the workspace's tail out for
+  int4* items;               // [max_items] {begin, end, flags, 0} of the merged sequence, then the edge partials:
+                             // [max_items][edge_levels][first | last][27] of runs that span items, and the same for
+                             // the diagonal (setup); the kernels find them from *max_items (op_edge_buffers)
+  int64_t m;                 // n_pos + n_nrm
+  int edge_levels;           // levels above the cut level
+  int walk_grid, edge_grid;  // persistent grids (multiples of the SM count)
 };
 
 // the operator over a workspace that nksr_op_setup prepared for the same hierarchy and constraints; NKSR_E_INVALID /
@@ -20,6 +36,6 @@ int mf_operator_make(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_
                      const int32_t* base_pos, const int32_t* base_nrm, void* ws, size_t ws_bytes, MfOperator* out);
 
 // y = A x.  pap != nullptr: also pap[b] = sum of x_i y_i over the rows of block b of a grid of exactly `blocks` blocks
-// of 256 threads (the fixed-order partials the PCG reduces).  done != nullptr: both kernels are no-ops once *done.
+// of 256 threads (the fixed-order partials the PCG reduces).  done != nullptr: every kernel is a no-op once *done.
 int mf_apply_launch(const MfOperator& op, const float* x, float* y, double* pap, int blocks, const int* done,
                     cudaStream_t s);

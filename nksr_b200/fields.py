@@ -37,6 +37,8 @@ BRICK_MIN_LOCATIONS_PER_VOXEL = 12.0
 # faster per bench.py step at 17.1 M unknowns (cfg4), 11 % slower at 2.0 M (cfg3, whose solve takes 16 iterations of an
 # operator that costs 2.5 packed SpMVs); the crossover between the two was not measured (DESIGN 4.2.1)
 MATRIX_FREE_MIN_UNKNOWNS = 8_000_000
+# locations per work item of the matrix-free gather-scatter (csrc/operator.cu; DESIGN 4.2.1)
+OP_ITEM_SIZE = 64
 
 
 _TOTAL_MEMORY = {}
@@ -49,16 +51,23 @@ def _total_memory(dev) -> int:
     return _TOTAL_MEMORY[key]
 
 
-def operator_bytes_per_apply(svh, n_pos: int, n_nrm: int, nrm_lines: int, channels: int) -> int:
+def operator_bytes_per_apply(svh, n_pos: int, n_nrm: int, nrm_lines: int, channels: int,
+                             item_size: int = OP_ITEM_SIZE) -> int:
     """Byte model of one matrix-free application of A (csrc/operator.cu), from shapes: the kernel rows (128 B per
-    location, level and line: nrm_lines = 1 compact, 3 full), the locations' containing voxels (4 B per level), nbr27
-    read once per voxel by each kernel, the planar partial sums written and gathered once (27 floats per voxel each),
-    the features z (4 C B per voxel) and x read twice and y written (12 B per voxel).  Voxels without locations are
-    counted as if they had some, so it is an upper bound of the algorithmic bytes.  bench.py's roofline_spmv
+    location, level and line: nrm_lines = 1 compact, 3 full), the merged location order and its containing voxels
+    (4 B per location and level, plus 4), the work items (16 B each) and their edge partials written and summed
+    (2 x 108 B per item and level above the cut), nbr27 read once per voxel by each kernel, the planar partial sums
+    written and gathered once (27 floats per voxel each), the features z (4 C B per voxel) and x read twice and y
+    written (12 B per voxel).  Voxels without locations are counted as if they had some, and the item count is its
+    bound 2 m / item_size + top voxels, so it is an upper bound of the algorithmic bytes.  bench.py's roofline_spmv
     (8 nnz + 12 n) describes the assembled matrix, not this path."""
     L, n = svh.depth, svh.num_unknowns
+    m = n_pos + n_nrm
     rows = 128 * L * (n_pos + nrm_lines * n_nrm)
-    return int(rows + 4 * L * (n_pos + n_nrm) + 2 * 108 * n + 2 * 108 * n + 4 * channels * n + 12 * n)
+    items = 2 * -(-m // item_size) + svh.num_voxels(L - 1)
+    edge_levels = max(L - 3, 0)                         # levels above the cut level 2
+    return int(rows + 4 * (L + 1) * m + items * (16 + 2 * 2 * 108 * edge_levels) + 2 * 108 * n + 2 * 108 * n
+               + 4 * channels * n + 12 * n)
 
 
 class EvaluationResult(SimpleNamespace):
@@ -107,9 +116,11 @@ def _as_level_list(features, depth):
     return [features[d] if d < len(features) else None for d in range(depth)]
 
 
-def _sorted_locations(svh: SparseFeatureHierarchy, xyz: torch.Tensor, extra: Optional[torch.Tensor] = None):
+def _sorted_locations(svh: SparseFeatureHierarchy, xyz: torch.Tensor, extra: Optional[torch.Tensor] = None,
+                      with_keys: bool = False):
     """Morton-sort locations and locate them on every level: (perm, sorted xyz, sorted extra, base (depth, m),
-    ranges (n, 2): the first / last + 1 sorted location of every voxel, levels concatenated)."""
+    ranges (n, 2): the first / last + 1 sorted location of every voxel, levels concatenated), and with `with_keys`
+    also their sorted half-voxel keys (m,) int64, the order the matrix-free operator merges by."""
     dev = xyz.device
     st = stream_ptr(dev)
     m = xyz.shape[0]
@@ -118,7 +129,7 @@ def _sorted_locations(svh: SparseFeatureHierarchy, xyz: torch.Tensor, extra: Opt
     call("nksr_point_half_keys", xyz, m, svh.voxel_size, hk, status, st)
     if int(status.item()) & 1:
         raise _lib.NksrError("constraint locations outside the supported range (|x| < 2^19 voxels) or non-finite")
-    _, perm = _lib.sort_pairs(hk, torch.arange(m, dtype=torch.int32, device=dev))
+    keys, perm = _lib.sort_pairs(hk, torch.arange(m, dtype=torch.int32, device=dev))
     perm = perm.long()
     xs = xyz[perm].contiguous()
     ex = extra[perm].contiguous() if extra is not None else None
@@ -128,7 +139,7 @@ def _sorted_locations(svh: SparseFeatureHierarchy, xyz: torch.Tensor, extra: Opt
     offs = svh.offsets
     for l in range(svh.depth):
         call("nksr_row_ranges", base[l], m, ranges[offs[l]:], svh.num_voxels(l), st)
-    return perm, xs, ex, base, ranges
+    return (perm, xs, ex, base, ranges, keys) if with_keys else (perm, xs, ex, base, ranges)
 
 
 _SIDE_STREAMS = {}
@@ -205,8 +216,8 @@ class KernelField(BaseField):
         return self._feat_view
 
     # ------------------------------------------------------------------ solve
-    def _sorted_locations(self, xyz: torch.Tensor, extra: Optional[torch.Tensor] = None):
-        return _sorted_locations(self.svh, xyz, extra)
+    def _sorted_locations(self, xyz: torch.Tensor, extra: Optional[torch.Tensor] = None, with_keys: bool = False):
+        return _sorted_locations(self.svh, xyz, extra, with_keys)
 
     def _sorted_rows(self, xyz: torch.Tensor, mode: int, extra: Optional[torch.Tensor] = None,
                      interleaved: bool = False, loc=None):
@@ -297,9 +308,11 @@ class KernelField(BaseField):
         return alpha
 
     def matrix_free_system(self, pos_xyz, normal_xyz=None, normal_value=None, pos_weight=1.0, normal_weight=1.0,
-                           reg_weight=1.0):
+                           reg_weight=1.0, item_size: Optional[int] = None):
         """Kernel rows of the sorted constraint locations and the operator's setup (nksr_op_setup): returns
-        .rhs, .diag, .n and what apply_operator needs (the rows, the constraint struct, the operator's workspace)."""
+        .rhs, .diag, .n and what apply_operator needs (the rows, the constraint struct, the operator's workspace).
+        item_size: at most that many locations per work item of the gather-scatter (default OP_ITEM_SIZE; see
+        operator_items)."""
         svh = self.svh
         dev = svh.device
         _lib.require_cuda(pos_xyz, "pos_xyz")
@@ -311,18 +324,18 @@ class KernelField(BaseField):
             raise _lib.NksrError("more than 2^31 unknowns: shard the cloud (chunk_size)")
         pos_xyz = pos_xyz.detach().to(dev, torch.float32).contiguous()
         cs = _lib.ConstraintsT()
-        loc_pos = self._sorted_locations(pos_xyz)
+        *loc_pos, key_pos = self._sorted_locations(pos_xyz, with_keys=True)
         _, _, base_pos, range_pos, e_pos = self._sorted_rows(pos_xyz, 0, loc=loc_pos)
         cs.e_pos, cs.range_pos, cs.n_pos, cs.w_pos = e_pos.data_ptr(), range_pos.data_ptr(), pos_xyz.shape[0], float(pos_weight)
-        keep = [e_pos, range_pos]
-        base_nrm, lines, K = None, 0, 0
+        keep = [e_pos, range_pos, key_pos]
+        base_nrm, key_nrm, lines, K = None, None, 0, 0
         if normal_xyz is not None and normal_xyz.shape[0] > 0:
             normal_xyz = normal_xyz.detach().to(dev, torch.float32).contiguous()
             normal_value = normal_value.detach().to(dev, torch.float32).contiguous()
             mode = 2 if self.approx_kernel_grad else 1          # compact lines: one 128 B line per location and level
-            loc_nrm = self._sorted_locations(normal_xyz, normal_value)
+            *loc_nrm, key_nrm = self._sorted_locations(normal_xyz, normal_value, with_keys=True)
             _, t_nrm, base_nrm, range_nrm, e_nrm = self._sorted_rows(normal_xyz, mode, normal_value, loc=loc_nrm)
-            keep += [t_nrm, range_nrm, e_nrm]
+            keep += [t_nrm, range_nrm, e_nrm, key_nrm]
             cs.e_nrm, cs.range_nrm, cs.t_nrm = e_nrm.data_ptr(), range_nrm.data_ptr(), t_nrm.data_ptr()
             K, lines = normal_xyz.shape[0], (1 if mode == 2 else 3)
             cs.n_nrm, cs.w_nrm, cs.nrm_compact = K, float(normal_weight), int(mode == 2)
@@ -333,15 +346,33 @@ class KernelField(BaseField):
         cs.mblocks, cs.split_level = None, svh.depth
         tm = getattr(self, "_timer", None) or _lib.StageTimer(dev, enabled=False)
         tm.mark("kernel_rows")
-        nb_op = call("nksr_op_workspace_bytes", svh.view())
+        S = int(item_size or OP_ITEM_SIZE)
+        if S < 1:
+            raise ValueError("item_size must be at least 1")
+        nb_op = call("nksr_op_workspace_bytes", svh.view(), cs, S)
         op_ws = torch.empty(nb_op, dtype=torch.uint8, device=dev)
         rhs = torch.empty(n, dtype=torch.float32, device=dev)
         diag = torch.empty(n, dtype=torch.float32, device=dev)
-        call("nksr_op_setup", svh.view(), self.feat_view(), cs, base_pos, base_nrm, rhs, diag, op_ws, nb_op, st)
+        call("nksr_op_setup", svh.view(), self.feat_view(), cs, base_pos, base_nrm, key_pos, key_nrm, S, rhs, diag,
+             op_ws, nb_op, st)
         tm.mark("operator_setup")
         return SimpleNamespace(cs=cs, base_pos=base_pos, base_nrm=base_nrm, rhs=rhs, diag=diag, ws=op_ws,
-                               ws_bytes=nb_op, n=n, keep=keep,
-                               bytes_per_apply=operator_bytes_per_apply(svh, pos_xyz.shape[0], K, lines, self.channels))
+                               ws_bytes=nb_op, n=n, keep=keep, item_size=S,
+                               bytes_per_apply=operator_bytes_per_apply(svh, pos_xyz.shape[0], K, lines, self.channels,
+                                                                        S))
+
+    def operator_items(self, op):
+        """The work of a matrix_free_system, from its workspace: (order, vox, items).  order (m,) int32 is the merged
+        location order (r >= 0: sorted position r, ~r: sorted normal location r), vox (depth, m) their containing
+        voxels, items (count, 4) int32 the work items: begin, end in order, flags (1: first, 2: last item of its
+        top-level voxel), 0.  Reads the item count back to the host."""
+        out = (C.c_int64 * 4)()
+        call("nksr_op_workspace_layout", self.svh.view(), op.cs, op.ws_bytes, C.addressof(out))
+        m = op.cs.n_pos + op.cs.n_nrm
+        i32 = lambda off, cnt: op.ws[off:off + 4 * cnt].view(torch.int32)
+        count = int(i32(out[2], 1).item())
+        return i32(out[0], m), i32(out[1], self.svh.depth * m).view(self.svh.depth, m), \
+            i32(out[3], 4 * count).view(count, 4)
 
     def apply_operator(self, op, x: torch.Tensor) -> torch.Tensor:
         """y = A x for a system of matrix_free_system (nksr_op_apply)"""
