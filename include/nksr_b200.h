@@ -435,6 +435,18 @@ NKSR_API int nksr_neural_interp(const nksr_svh_t* svh, const nksr_feat_t* feat, 
  * sum_q T3(q) grad[q]; the others are not touched.  Deterministic: no atomics, one fixed summation order. */
 NKSR_API int nksr_neural_interp_vjp(const nksr_svh_t* svh, int channels, int level_mask, const float* xyz,
                                     const int32_t* range, int64_t m, const float* grad, float* dfeat, void* stream);
+/* the position Jacobian of nksr_neural_interp (SPEC S17a): jac (m x 3 x C*popcount(level_mask), every entry written)
+ * holds jac[i][a][g*C + c] = d out[i][g*C + c] / dx_a, from the tent derivative of SPEC S4 (one-sided in the
+ * containing cell, symmetric in the snap zone |tau| < 2^-12) divided by W_l; a row is 0 wherever out is.  out
+ * (nullable): when given, written bitwise as nksr_neural_interp writes it. */
+NKSR_API int nksr_neural_interp_jacobian(const nksr_svh_t* svh, const nksr_feat_t* feat, int level_mask,
+                                         const float* xyz, int64_t m, float* out, float* jac, void* stream);
+/* its VJP with respect to the features, under the conventions of nksr_neural_interp_vjp: grad (m x 3 x
+ * C*popcount(level_mask)) in the sorted order; the blocks of the given levels of dfeat are OVERWRITTEN with
+ * sum_q sum_a dT3_a(q) / W_l grad[q][a]. */
+NKSR_API int nksr_neural_interp_jacobian_vjp(const nksr_svh_t* svh, int channels, int level_mask, const float* xyz,
+                                             const int32_t* range, int64_t m, const float* grad, float* dfeat,
+                                             void* stream);
 
 /* ---- f1: nksr.get_estimate_normal_preprocess_fn (examples/recons_waymo.py:36; CPU twin
  *      examples/recons_waymo_cpu.py:21-41): voxel-neighbourhood PCA normals ---- */
@@ -486,7 +498,7 @@ NKSR_API int nksr_sdf_from_points(const nksr_svh_t* svh, const float* xyz, const
                          int nb_points, float stdv, int imls, int start_level, float* sdf, float* grad,
                          void* stream);
 
-/* ---- metrics.MeshEvaluator (models/nksr_net.py:298-312; DESIGN.md SPEC S18).
+/* ---- metrics.MeshEvaluator (models/nksr_net.py:298-312; DESIGN.md SPEC S17a).
  * nksr_sample_surface: n area-uniform samples of the mesh (v: float[V*3], f: int32[n_tri*3]).  start: int64[n_tri+1],
  * the first sample of every triangle (start[0] = 0, start[n_tri] = n, non-decreasing; the caller forms it from the
  * fp64 area prefix).  Sample i lies on triangle out_tri[i] at the barycentrics of a counter hash of (seed, i);

@@ -133,6 +133,8 @@ _SIGNATURES = {
     "nksr_layer_mask": ("i", "Spqipp"),
     "nksr_neural_interp": ("i", "SFipqpp"),
     "nksr_neural_interp_vjp": ("i", "Siippqppp"),
+    "nksr_neural_interp_jacobian": ("i", "SFipqppp"),
+    "nksr_neural_interp_jacobian_vjp": ("i", "Siippqppp"),
     "nksr_voxel_moments": ("i", "pqppfpp"),
     "nksr_voxel_pca_normals": ("i", "ppqfpp"),
     "nksr_orient_normals": ("i", "ppppqfppp"),

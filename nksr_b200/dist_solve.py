@@ -292,6 +292,10 @@ def reconstruct_global(reconstructor, xyz: torch.Tensor, normal: Optional[torch.
         # every rank would grow its own hierarchy from its own predictions, which can disagree in the halo
         raise _lib.NksrError("the global solve needs structure='encoder': hierarchies grown from the predicted "
                              "structure are not kept consistent across ranks")
+    if getattr(reconstructor.network, "geometry", "kernel") == "neural":
+        # the global solve is a kernel solve; a neural output field has nothing to solve
+        raise _lib.NksrError("the global solve does not support geometry='neural': build the network with "
+                             "geometry='kernel'")
     if getattr(reconstructor.network, "udf_enabled", False):
         # the sharded field is masked per slab by LayerField; there is no UDF hierarchy across ranks
         raise _lib.NksrError("the global solve does not support udf.enabled: build the network with "

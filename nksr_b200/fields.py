@@ -93,6 +93,13 @@ class BaseField:
     def evaluate_f(self, xyz: torch.Tensor, grad: bool = False) -> EvaluationResult:
         raise NotImplementedError
 
+    def evaluate_f_bar(self, xyz: torch.Tensor) -> torch.Tensor:
+        """Occupancy-style value (> 0 inside, models/loss.py:99); masked-out regions read as outside."""
+        f = self.evaluate_f(xyz).value
+        if self.mask_field is not None:
+            f = torch.where(self.mask_field.mask(xyz), f, -f.abs())
+        return f
+
     def mask(self, xyz: torch.Tensor) -> torch.Tensor:
         """bool (M,): True where geometry is kept by this field used as a mask."""
         raise NotImplementedError
@@ -672,13 +679,6 @@ class KernelField(BaseField):
         offs = self.svh.offsets
         return tuple(dz[offs[l]:offs[l] + self.svh.num_voxels(l)] for l in range(self.svh.depth))
 
-    def evaluate_f_bar(self, xyz: torch.Tensor) -> torch.Tensor:
-        """Occupancy-style value (> 0 inside, models/loss.py:99); masked-out regions read as outside."""
-        f = self.evaluate_f(xyz).value
-        if self.mask_field is not None:
-            f = torch.where(self.mask_field.mask(xyz), f, -f.abs())
-        return f
-
     def mask(self, xyz):
         return self.evaluate_f(xyz).value >= self.level_set
 
@@ -807,15 +807,24 @@ class LayerField(BaseField):
 
 
 class NeuralField(BaseField):
-    """MLP-decoded field over trilinearly interpolated voxel features (the UDF mask, models/nksr_net.py:124-130; SPEC
-    S17): f(x) = decoder(u(x)), u(x) = the interpolated features of every given level (a level with features, empty or
-    not) in ascending order, C columns each.  The interpolation and its VJP are CUDA (csrc/neural_field.cu); the
-    decoder is a PyTorch module.  When grad is enabled and the features or the decoder's parameters require grad, the
-    values carry a graph into both (queries get no gradient)."""
+    """MLP-decoded field over trilinearly interpolated voxel features (the UDF mask, models/nksr_net.py:124-130, and the
+    output field of geometry='neural', :114-119; SPEC S17): f(x) = decoder(u(x)), u(x) = the interpolated features of
+    every given level (a level with features, empty or not) in ascending order, C columns each.  The interpolation and
+    its VJP are CUDA (csrc/neural_field.cu); the decoder is a PyTorch module.  When grad is enabled and the features or
+    the decoder's parameters require grad, the values carry a graph into both (queries get no gradient).
 
-    def __init__(self, svh: SparseFeatureHierarchy, decoder, features):
+    position_gradient: evaluate_f(xyz, grad=True) also returns grad f = sum_k (d decoder / d u_k)(u) J_k with J = du/dx
+    (SPEC S17a, nksr_neural_interp_jacobian).  The decoder's Jacobian is taken with torch.autograd.grad of the sum of its
+    outputs with respect to u, which assumes that the decoder acts on every row of u on its own (as the Linear / ReLU
+    MLPs here do).  When grad is enabled and the features or the decoder's parameters require grad, the gradient keeps
+    its graph (create_graph), so a loss on it reaches both: torch differentiates the decoder twice, and the CUDA nodes
+    (_NeuralInterp for u, _NeuralJacobian for J) only need their first-order VJPs.  Without it (the default) the field
+    is value-only and `gradient` is None."""
+
+    def __init__(self, svh: SparseFeatureHierarchy, decoder, features, position_gradient: bool = False):
         super().__init__(svh)
         self.decoder = decoder
+        self.position_gradient = bool(position_gradient)
         self.features = _as_level_list(features, svh.depth)
         given = [l for l, f in enumerate(self.features) if f is not None]
         if not given:
@@ -833,37 +842,63 @@ class NeuralField(BaseField):
         self.levels = given
         self.level_mask = sum(1 << l for l in given)
 
-    def interpolate(self, xyz: torch.Tensor) -> torch.Tensor:
-        """u(x), (M, C * len(levels)) fp32 (nksr_neural_interp); differentiable in the features when grad is enabled
-        and they require grad"""
+    def _inputs(self, xyz):
         _lib.require_cuda(xyz, "xyz")
         xyz = xyz.detach().to(self.svh.device, torch.float32).contiguous()
         feats = [f.to(self.svh.device, torch.float32).contiguous() if f is not None else None for f in self.features]
-        if torch.is_grad_enabled() and any(f is not None and f.requires_grad for f in feats):
+        return xyz, feats, torch.is_grad_enabled() and any(f is not None and f.requires_grad for f in feats)
+
+    def interpolate(self, xyz: torch.Tensor) -> torch.Tensor:
+        """u(x), (M, C * len(levels)) fp32 (nksr_neural_interp); differentiable in the features when grad is enabled
+        and they require grad"""
+        xyz, feats, graph = self._inputs(xyz)
+        if graph:
             return _NeuralInterp.apply(self, xyz, *feats)
         return self._interp_cuda(xyz, feats)
 
-    def _interp_cuda(self, xyz, feats):
-        m = xyz.shape[0]
-        out = torch.empty((m, self.channels * len(self.levels)), dtype=torch.float32, device=xyz.device)
+    def jacobian(self, xyz: torch.Tensor) -> torch.Tensor:
+        """J = du/dx, (M, 3, C * len(levels)) fp32 (nksr_neural_interp_jacobian, SPEC S17a): J[i][a] = d u(x_i) / dx_a;
+        differentiable in the features when grad is enabled and they require grad"""
+        xyz, feats, graph = self._inputs(xyz)
+        if graph:
+            return _NeuralJacobian.apply(self, xyz, *feats)
+        return self._jacobian_cuda(xyz, feats)
+
+    def _feat_view(self, feats):
         fv = _lib.FeatT()
         fv.channels = self.channels
         for l, f in enumerate(feats):
             fv.z[l] = f.data_ptr() if f is not None and f.shape[0] > 0 else None
-        call("nksr_neural_interp", self.svh.view(), fv, self.level_mask, xyz, m, out, stream_ptr(xyz.device))
+        return fv
+
+    def _interp_cuda(self, xyz, feats):
+        m = xyz.shape[0]
+        out = torch.empty((m, self.channels * len(self.levels)), dtype=torch.float32, device=xyz.device)
+        call("nksr_neural_interp", self.svh.view(), self._feat_view(feats), self.level_mask, xyz, m, out,
+             stream_ptr(xyz.device))
         return out
 
-    def _interp_vjp(self, xyz, g):
-        """dL/dF_l for every level (None where not given) from g = dL/du (nksr_neural_interp_vjp): the queries with a
-        containing voxel are Morton sorted and gathered per voxel, in one fixed order"""
+    def _jacobian_cuda(self, xyz, feats, with_values: bool = False):
+        """J, or (u, J) from the same pass with `with_values` (u bitwise what _interp_cuda gives)"""
+        m, w = xyz.shape[0], self.channels * len(self.levels)
+        jac = torch.empty((m, 3, w), dtype=torch.float32, device=xyz.device)
+        u = torch.empty((m, w), dtype=torch.float32, device=xyz.device) if with_values else None
+        call("nksr_neural_interp_jacobian", self.svh.view(), self._feat_view(feats), self.level_mask, xyz, m, u, jac,
+             stream_ptr(xyz.device))
+        return (u, jac) if with_values else jac
+
+    def _interp_vjp(self, xyz, g, jacobian: bool = False):
+        """dL/dF_l for every level (None where not given) from g = dL/du (nksr_neural_interp_vjp), or with `jacobian`
+        from g = dL/dJ, (M, 3, C * len(levels)) (nksr_neural_interp_jacobian_vjp): the queries with a containing voxel
+        are Morton sorted and gathered per voxel, in one fixed order"""
         svh, dev = self.svh, xyz.device
         dz = torch.zeros((svh.num_unknowns, self.channels), dtype=torch.float32, device=dev)
         if svh.num_unknowns > 0 and xyz.shape[0] > 0:
             keep = torch.nonzero(svh.locate(xyz)[svh.depth - 1] >= 0).reshape(-1)
             perm, xs, _, _, ranges = _sorted_locations(svh, xyz[keep].contiguous())
             gs = g.detach().to(torch.float32)[keep[perm]].contiguous()
-            call("nksr_neural_interp_vjp", svh.view(), self.channels, self.level_mask, xs, ranges, xs.shape[0], gs, dz,
-                 stream_ptr(dev))
+            call("nksr_neural_interp_jacobian_vjp" if jacobian else "nksr_neural_interp_vjp", svh.view(), self.channels,
+                 self.level_mask, xs, ranges, xs.shape[0], gs, dz, stream_ptr(dev))
         offs = svh.offsets
         return tuple(dz[offs[l]:offs[l] + svh.num_voxels(l)] if l in self.levels else None for l in range(svh.depth))
 
@@ -900,9 +935,26 @@ class NeuralField(BaseField):
         return out
 
     def evaluate_f(self, xyz, grad=False):
-        """f at xyz; `gradient` is None (the field has no position gradient here)"""
-        v = self.decoder(self.interpolate(xyz)).reshape(-1)
-        return EvaluationResult(value=v, gradient=None)
+        """f at xyz; with `grad` and position_gradient also grad f (M, 3), else `gradient` is None"""
+        if not (grad and self.position_gradient):
+            v = self.decoder(self.interpolate(xyz)).reshape(-1)
+            return EvaluationResult(value=v, gradient=None)
+        xyz, feats, feat_graph = self._inputs(xyz)
+        graph = feat_graph or (torch.is_grad_enabled() and any(
+            p.requires_grad for p in getattr(self.decoder, "parameters", lambda: [])()))
+        if feat_graph:
+            u, jac = _NeuralInterp.apply(self, xyz, *feats), _NeuralJacobian.apply(self, xyz, *feats)
+        else:
+            u, jac = self._jacobian_cuda(xyz, feats, with_values=True)
+        with torch.enable_grad():
+            if not graph or not u.requires_grad:
+                u = u.detach().requires_grad_(True)
+            v = self.decoder(u).reshape(-1)
+            (du,) = torch.autograd.grad(v.sum(), u, create_graph=graph)
+        g = torch.einsum("mk,mak->ma", du, jac)
+        if not graph:
+            v = v.detach()
+        return EvaluationResult(value=v, gradient=g)
 
     def mask(self, xyz):
         # UDF semantics: keep geometry closer than the level set to the data
@@ -928,6 +980,23 @@ class _NeuralInterp(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g):
         dfeat = ctx.field._interp_vjp(ctx.xyz, g)
+        ctx.field = ctx.xyz = None
+        return (None, None) + tuple(d if need else None for d, need in zip(dfeat, ctx.needs_input_grad[2:]))
+
+
+class _NeuralJacobian(torch.autograd.Function):
+    """J = du/dx (F, xyz).  Forward: nksr_neural_interp_jacobian.  Backward: dL/dF_l = sum_q sum_a dT3_a(q) / W_l
+    dL/dJ_q,a,l (nksr_neural_interp_jacobian_vjp); the queries get no gradient.  J is linear in F, so this VJP is the
+    whole derivative: no CUDA op needs a second derivative."""
+
+    @staticmethod
+    def forward(ctx, field, xyz, *feats):
+        ctx.field, ctx.xyz = field, xyz
+        return field._jacobian_cuda(xyz, feats)
+
+    @staticmethod
+    def backward(ctx, g):
+        dfeat = ctx.field._interp_vjp(ctx.xyz, g, jacobian=True)
         ctx.field = ctx.xyz = None
         return (None, None) + tuple(d if need else None for d, need in zip(dfeat, ctx.needs_input_grad[2:]))
 

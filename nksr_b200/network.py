@@ -34,9 +34,11 @@ from .svh import SparseFeatureHierarchy
 _DEFAULTS = dict(kernel_dim=4, tree_depth=4, adaptive_depth=2, feature="normal",
                  interpolator=dict(n_hidden=2, hidden_dim=16), udf=dict(enabled=False), seed=0,
                  unet=dict(f_maps=32), backbone="pool", precision="fp32", trainable=False, structure="encoder",
-                 structure_max_ratio=None)
+                 structure_max_ratio=None, geometry="kernel")
 # the UDF decoder of udf.enabled draws its initial weights from seed + this offset
 UDF_DECODER_SEED_OFFSET = 0x5D17
+# the SDF decoder of geometry='neural' draws its initial weights from seed + this offset
+SDF_DECODER_SEED_OFFSET = 0x5DF0
 
 
 def _get(hp, key, default):
@@ -104,6 +106,14 @@ class NKSRNetwork(nn.Module):
         self.udf_enabled = bool(_get(hp["udf"], "enabled", False))
         if self.udf_enabled and self.backbone != "unet":
             raise ValueError("udf.enabled needs backbone='unet' (the 'pool' stand-in has no UDF head)")
+        # geometry: the output field of a reconstruction (models/nksr_net.py:89-122).  'kernel' = the KernelField solved
+        # from the basis features; 'neural' = the NeuralField sdf_decoder(u(x)) over the basis features of every decoder
+        # level (no solve) -- U-Net backbone only
+        self.geometry = str(hp["geometry"])
+        if self.geometry not in ("kernel", "neural"):
+            raise ValueError(f"geometry: 'kernel' or 'neural', not {self.geometry!r}")
+        if self.geometry == "neural" and self.backbone != "unet":
+            raise ValueError("geometry='neural' needs backbone='unet' (the 'pool' stand-in has no decoder to train)")
         interp = hp["interpolator"]
         gen = torch.Generator().manual_seed(int(hp["seed"]))
         state = torch.random.get_rng_state()
@@ -129,6 +139,12 @@ class NKSRNetwork(nn.Module):
                 # is bitwise what it is with udf disabled (the Linear(C, 16) above only keeps the draws in step)
                 torch.manual_seed(int(hp["seed"]) + UDF_DECODER_SEED_OFFSET)
                 self.udf_decoder = nn.Sequential(nn.Linear(C * self.tree_depth, 32), nn.ReLU(), nn.Linear(32, 32),
+                                                 nn.ReLU(), nn.Linear(32, 1))
+            if self.geometry == "neural":
+                # the decoder of the neural output field, C columns per level; built after every other module from its
+                # own seed, like the UDF decoder, so that every other parameter is bitwise that of geometry='kernel'
+                torch.manual_seed(int(hp["seed"]) + SDF_DECODER_SEED_OFFSET)
+                self.sdf_decoder = nn.Sequential(nn.Linear(C * self.tree_depth, 32), nn.ReLU(), nn.Linear(32, 32),
                                                  nn.ReLU(), nn.Linear(32, 1))
         finally:
             torch.random.set_rng_state(state)

@@ -336,7 +336,7 @@ class Reconstructor:
 
     # one chunk / the whole cloud: models/nksr_net.py:41-133 without the Lightning plumbing
     def _reconstruct_one(self, xyz, normal, sensor, voxel_size, approx_kernel_grad, solver_tol, fused_mode,
-                         solver_max_iter) -> KernelField:
+                         solver_max_iter) -> BaseField:
         if normal is not None:
             feat = normal
         elif sensor is not None:
@@ -356,12 +356,18 @@ class Reconstructor:
         feats, dec_svh, udf_svh = self.network.unet(enc, svh, adaptive_depth=self.adaptive_depth)
         if getattr(self.network, "structure", "encoder") == "predicted" and dec_svh.num_unknowns == 0:
             raise _lib.NksrError("predicted structure is empty: the network kept no voxel, there is nothing to solve")
+        ad = min(self.adaptive_depth, dec_svh.depth)
+        if getattr(self.network, "geometry", "kernel") == "neural":
+            # models/nksr_net.py:114-119: the output field is the SDF decoder over the basis features, no solve
+            field = NeuralField(dec_svh, self.network.sdf_decoder, feats.basis_features, position_gradient=True)
+            tm.mark("network")
+            field.set_mask_field(mask_field(self.network, feats, dec_svh, udf_svh, ad, voxel_size))
+            return field
         field = KernelField(dec_svh, self.network.interpolators, feats.basis_features, approx_kernel_grad)
         field._timer = tm
         tm.mark("network")
         field.solver_config["tol"] = float(solver_tol)
         field.solver_config["max_iter"] = int(solver_max_iter)
-        ad = min(self.adaptive_depth, dec_svh.depth)
         normal_xyz = torch.cat([dec_svh.get_voxel_centers(d) for d in range(ad)])
         normal_value = torch.cat([feats.normal_features[d] for d in range(ad)])
         normal_weight = NORMAL_WEIGHT / normal_xyz.shape[0] * (voxel_size ** 2)        # models/nksr_net.py:103-104
@@ -399,8 +405,11 @@ class Reconstructor:
             voxel_size = DEFAULT_VOXEL_SIZE if detail_level is None else voxel_size_from_detail(xyz, detail_level)
         field = self._reconstruct_one(xyz, normal, sensor, float(voxel_size), approx_kernel_grad, solver_tol,
                                       fused_mode, solver_max_iter)
-        self.last_stats = dict(field.solve_info, voxel_size=float(voxel_size), points=int(xyz.shape[0]),
-                               normal_locations=int(getattr(field, "_n_normal", 0)))
+        if isinstance(field, NeuralField):
+            self.last_stats = dict(voxel_size=float(voxel_size), points=int(xyz.shape[0]), geometry="neural")
+        else:
+            self.last_stats = dict(field.solve_info, voxel_size=float(voxel_size), points=int(xyz.shape[0]),
+                                   normal_locations=int(getattr(field, "_n_normal", 0)))
         return field
 
     def stage_times(self) -> dict:
@@ -409,6 +418,11 @@ class Reconstructor:
 
     def _reconstruct_chunks(self, xyz, normal, sensor, voxel_size, chunk_size, preprocess_fn, approx_kernel_grad,
                             solver_tol, fused_mode, solver_max_iter, chunk_filter=None):
+        if getattr(self.network, "geometry", "kernel") == "neural":
+            # (also reached from dist.reconstruct_distributed) the chunks are blended as solved kernel fields
+            raise _lib.NksrError("chunk mode does not support geometry='neural': the blended chunk field is built from "
+                                 "kernel solves; build the network with geometry='kernel' or reconstruct without "
+                                 "chunk_size")
         if getattr(self.network, "udf_enabled", False):
             # (also reached from dist.reconstruct_distributed) the blended field has no UDF hierarchy to mask with
             raise _lib.NksrError("chunk mode does not support udf.enabled: the blended chunk field has no UDF "

@@ -2,7 +2,9 @@
 and :106-140), with the samplers and ground-truth transform of configs/default/train.yaml
 (supervision.structure_weight, supervision.udf, supervision.spatial.gt_band / gt_soft), and -- opt-in,
 `train_step(..., kernel=True)` -- the kernel-field losses, which backpropagate through the kernel solve
-(supervision.gt_surface and supervision.spatial, models/loss.py:163-260; fields._KernelSolve).
+(supervision.gt_surface and supervision.spatial, models/loss.py:163-260; fields._KernelSolve), or with
+geometry='neural' the same losses on the NeuralField output field, whose normal loss backpropagates through its position
+gradient (fields._NeuralJacobian).
 
     feat, dec_svh, _ = net.unet(net.encoder(xyz, normal, svh, 0), svh)
     l_struct, per_level = structure_loss(feat.structure_features, dec_svh, gt_svh)
@@ -186,13 +188,24 @@ def spatial_loss(field, ref_xyz, ref_normal, voxel_size, samplers=SPATIAL_SAMPLE
     return torch.sum(torch.abs((pd - gt) / voxel_size)) / q.shape[0]
 
 
+def neural_field(net, feat, dec_svh: SparseFeatureHierarchy):
+    """the output field of geometry='neural' (models/nksr_net.py:114-119): the SDF decoder over the basis features of
+    every level, with its position gradient; differentiable in both when grad is enabled.  The interpolators and the
+    normal features are not used."""
+    return NeuralField(dec_svh, net.sdf_decoder, feat.basis_features, position_gradient=True)
+
+
 def kernel_losses(net, scene: TrainingScene, generator=None, feat=None, dec_svh=None, timer=None):
-    """the kernel-field losses of a trainable NKSRNetwork on the scene: dict(total, gt_value, gt_normal, spatial,
-    field).  `feat`, `dec_svh`: an existing forward of the network (else one is run)."""
+    """the field losses of a trainable NKSRNetwork on the scene: dict(total, gt_value, gt_normal, spatial, field), on
+    the KernelField (kernel_field), or with geometry='neural' on the NeuralField (neural_field, no solve).  `feat`,
+    `dec_svh`: an existing forward of the network (else one is run)."""
     if feat is None:
         enc = net.encoder(scene.xyz, scene.normal, scene.enc_svh, 0)
         feat, dec_svh, _ = net.unet(enc, scene.enc_svh, adaptive_depth=scene.adaptive_depth)
-    field = kernel_field(net, feat, dec_svh, scene, timer)
+    if getattr(net, "geometry", "kernel") == "neural":
+        field = neural_field(net, feat, dec_svh)
+    else:
+        field = kernel_field(net, feat, dec_svh, scene, timer)
     l_val, l_nrm = gt_surface_loss(field, scene.xyz, scene.normal, generator=generator)
     l_sp = spatial_loss(field, scene.xyz, scene.normal, scene.voxel_size, generator=generator)
     total = GT_SURFACE_VALUE_WEIGHT * l_val + GT_SURFACE_NORMAL_WEIGHT * l_nrm + SPATIAL_WEIGHT * l_sp

@@ -6,6 +6,7 @@ the structure and UDF losses (nksr_b200/training.py), Adam lr 1e-4, gradient nor
     python tools/train_unet.py --scene cfg4 --points 1000000 --depth 4 --kernel-losses --steps 10
     python tools/train_unet.py --scene cfg4 --points 1000000 --depth 4 --structure predicted --steps 10
     python tools/train_unet.py --scene cfg4 --points 1000000 --depth 4 --udf --steps 10
+    python tools/train_unet.py --scene sphere --points 200000 --depth 4 --geometry neural --steps 30
 
 Scenes: 'sphere' (tests/clouds.py, exact normals) or 'cfg4' (a crop of bench.py's outdoor scene at its own density,
 normals from the kNN preprocess).  Every step prints one JSON line: the losses and the CUDA-event times of the forward,
@@ -19,6 +20,8 @@ kernels (with the field evaluations they need).
 from the prediction with probability --pd-structure-prob); after training one more line reports, per level, the
 structure accuracy and the sizes |E_l| (encoder), |T_l| (grown) and |dec_l| (kept), the CUDA-event time of every growth
 step and the backbone's forward time on the encoder hierarchy against the grown one under teacher forcing.
+--geometry neural builds the network with geometry='neural': the field losses (implied) are taken on the NeuralField
+output field sdf_decoder(u(x)), whose normal loss trains through its position gradient (no solve).
 --udf builds the network with udf.enabled: the UDF loss is the NeuralField's over every level of the decoder hierarchy,
 through the interpolation kernels (csrc/neural_field.cu), instead of the finest level's alone.
 --out saves {'state_dict': ...}, which load_checkpoint_from_url(<path>) + load_state_dict take."""
@@ -163,7 +166,11 @@ def main(argv=None):
                     help="--structure predicted: probability of growing from the prediction instead of teacher forcing")
     ap.add_argument("--udf", action="store_true",
                     help="udf.enabled: the UDF loss on the NeuralField over every level (DESIGN.md SPEC S17)")
+    ap.add_argument("--geometry", choices=("kernel", "neural"), default="kernel",
+                    help="output field: the kernel solve, or the NeuralField sdf_decoder(u(x)) (implies --kernel-losses)")
     args = ap.parse_args(argv)
+    if args.geometry == "neural":
+        args.kernel_losses = True
     if args.steps < 1:
         ap.error("--steps must be >= 1")
     import torch
@@ -179,13 +186,13 @@ def main(argv=None):
     scene = make_scene(args.scene, args.points, args.depth, dev)
     net = NKSRNetwork(dict(backbone="unet", tree_depth=args.depth, kernel_dim=4, precision=args.precision,
                            trainable=True, seed=args.seed, structure=args.structure,
-                           udf=dict(enabled=args.udf))).to(dev)
+                           udf=dict(enabled=args.udf), geometry=args.geometry)).to(dev)
     opt = T.make_optimizer(net)
     gen = torch.Generator(device=dev).manual_seed(args.seed)
     timer = KernelTimer(U)
     info = dict(gpu_info(0), scene=args.scene, points=int(scene.xyz.shape[0]), voxel_size=scene.voxel_size,
                 depth=args.depth, precision=args.precision, structure=args.structure,
-                pd_structure_prob=args.pd_structure_prob, udf=args.udf,
+                pd_structure_prob=args.pd_structure_prob, udf=args.udf, geometry=args.geometry,
                 voxels=[scene.enc_svh.num_voxels(l) for l in range(args.depth)])
     print(json.dumps(dict(setup=info)), flush=True)
     rows = []
