@@ -516,6 +516,19 @@ NKSR_API int nksr_metric_nearest(const nksr_svh_t* svh, const float* xyz, const 
                         const float* origin3, int start_level, float* out_dist, int32_t* out_idx, float* out_dot,
                         int32_t* far_list, int32_t* far_count, void* stream);
 
+/* ---- PointTSDFVolume ground truth from sensor rays (groundtruth.bin, dataset/av.py:94; consumed by
+ * dataset/av_gt_geometry.py:141-173 and models/loss.py:221-249; DESIGN.md SPEC S19).
+ * Ray j runs from sensor[j] to xyz[j] (float[n*3] each; rays with a non-finite input or zero length are skipped).
+ * Node (i, j, k) sits at volume_min3 + (i, j, k) h (host float[3], evaluated in fp64); dims3 (host int64[3]) >= 2
+ * each, product < 2^31; h > 0, tau > 0.  volume (float[dims0*dims1*dims2], [X][Y][Z]) = sdf / tau of the near observation with the
+ * smallest |sdf| < tau (ties: the lower ray index), else +1 where a ray passed with sdf >= tau before reaching any
+ * near node, else NaN.  Bitwise repeatable; the classes do not depend on the order of the rays.
+ * ws: nksr_tsdf_volume_workspace_bytes(dims3) bytes (one 64-bit key per node; 0 for invalid dims), else
+ * NKSR_E_WORKSPACE. */
+NKSR_API size_t nksr_tsdf_volume_workspace_bytes(const int64_t* dims3);
+NKSR_API int nksr_tsdf_volume(const float* xyz, const float* sensor, int64_t n, const float* volume_min3, float h,
+                              const int64_t* dims3, float tau, float* volume, void* ws, size_t ws_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

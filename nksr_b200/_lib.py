@@ -144,6 +144,8 @@ _SIGNATURES = {
     "nksr_sdf_from_points": ("i", "Sppppqppqifiippp"),
     "nksr_sample_surface": ("i", "ppqpqqpppp"),
     "nksr_metric_nearest": ("i", "Spppp" + "qppqpi" + "pppppp"),
+    "nksr_tsdf_volume_workspace_bytes": ("z", "p"),
+    "nksr_tsdf_volume": ("i", "ppqpfpfppzp"),
 }
 
 _lib = None

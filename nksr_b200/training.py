@@ -102,36 +102,40 @@ def udf_samples(svh, ref_xyz, ref_normal, voxel_size, samplers=UDF_SAMPLERS, gen
     return torch.cat(out, 0)
 
 
-def udf_gt(q, ref_xyz, ref_normal, voxel_size, gt_band=GT_BAND):
-    """|transform(-sdf_from_points(q, ref, 8, 0.02))| (models/loss.py:84-86, 111-118)"""
+def udf_gt(q, ref_xyz, ref_normal, voxel_size, gt_band=GT_BAND, gt=None):
+    """|transform(-sdf_from_points(q, ref, 8, 0.02))|, or with volume ground truth (a PointTSDFVolume)
+    |transform(gt.query_sdf(q))| (models/loss.py:84-86, 111-118)"""
+    if gt is not None:
+        return transform_field(gt.query_sdf(q), voxel_size, gt_band).abs()
     sdf = -sdf_from_points(q, ref_xyz, ref_normal, 8, 0.02, False)[0]
     return transform_field(sdf, voxel_size, gt_band).abs()
 
 
 def udf_loss(udf_decoder, udf_features, svh: SparseFeatureHierarchy, ref_xyz, ref_normal, voxel_size,
-             samplers=UDF_SAMPLERS, gt_band=GT_BAND, generator=None, q=None):
+             samplers=UDF_SAMPLERS, gt_band=GT_BAND, generator=None, q=None, gt=None):
     """mean |transform(pd) - gt| / voxel_size over the UDF samples (models/loss.py:120-140).  pd is the UDF NeuralField
     evaluated differentiably as udf_decoder(NeuralField._interp(q)) on the finest level's UDF features (the decoder
-    takes kernel_dim inputs); `q` overrides the samplers.  Zero when the finest level is empty (a hierarchy grown from
-    a prediction that kept nothing there): there is no field to evaluate."""
+    takes kernel_dim inputs); `q` overrides the samplers; `gt` (a PointTSDFVolume) gives the ground truth (udf_gt).
+    Zero when the finest level is empty (a hierarchy grown from a prediction that kept nothing there): there is no
+    field to evaluate."""
     if svh.num_voxels(0) == 0:
         return torch.zeros((), device=svh.device)
     if q is None:
         q = udf_samples(svh, ref_xyz, ref_normal, voxel_size, samplers, generator)
-    gt = udf_gt(q, ref_xyz, ref_normal, voxel_size, gt_band)
+    gt = udf_gt(q, ref_xyz, ref_normal, voxel_size, gt_band, gt)
     field = NeuralField(svh, udf_decoder, {0: udf_features[0]})
     pd = udf_decoder(field._interp(q.to(torch.float32).contiguous())).reshape(-1)
     return torch.mean((transform_field(pd, voxel_size, gt_band) - gt).abs()) / voxel_size
 
 
 def udf_field_loss(udf_decoder, udf_features, svh: SparseFeatureHierarchy, ref_xyz, ref_normal, voxel_size,
-                   samplers=UDF_SAMPLERS, gt_band=GT_BAND, generator=None, q=None):
+                   samplers=UDF_SAMPLERS, gt_band=GT_BAND, generator=None, q=None, gt=None):
     """the UDF loss of udf.enabled (models/loss.py:120-140): the same samples, ground truth and L1 as `udf_loss`, but pd
     is the UDF NeuralField over every level of `svh` (the decoder takes kernel_dim columns per level), evaluated and
     backpropagated through the interpolation kernels (csrc/neural_field.cu)"""
     if q is None:
         q = udf_samples(svh, ref_xyz, ref_normal, voxel_size, samplers, generator)
-    gt = udf_gt(q, ref_xyz, ref_normal, voxel_size, gt_band)
+    gt = udf_gt(q, ref_xyz, ref_normal, voxel_size, gt_band, gt)
     field = NeuralField(svh, udf_decoder, udf_features)
     pd = field.evaluate_f(q.to(torch.float32).contiguous()).value
     return torch.mean((transform_field(pd, voxel_size, gt_band) - gt).abs()) / voxel_size
@@ -140,14 +144,19 @@ def udf_field_loss(udf_decoder, udf_features, svh: SparseFeatureHierarchy, ref_x
 class TrainingScene:
     """one oriented cloud with its encoder hierarchy (point splatting) and ground-truth hierarchy (adaptive, from the
     normals, models/nksr_net.py:175-179).  The decoder runs on the encoder hierarchy: the predicted-structure regime,
-    where all three structure classes occur."""
+    where all three structure classes occur.  `gt`: volume ground truth (a gt_geometry.PointTSDFVolume on the same
+    device); every loss then takes its reference from it, as models/nksr_net.py and models/loss.py do with
+    DS.GT_GEOMETRY: the ground-truth hierarchy and the surface samples from gt.xyz / gt.normal, the SDF from
+    gt.query_sdf and the spatial loss's empty-space term from gt.query_classification."""
 
-    def __init__(self, xyz, normal, voxel_size, depth, adaptive_depth=2):
+    def __init__(self, xyz, normal, voxel_size, depth, adaptive_depth=2, gt=None):
         dev = xyz.device
         self.xyz, self.normal, self.voxel_size = xyz.contiguous(), normal.contiguous(), float(voxel_size)
+        self.gt = gt
+        self.ref_xyz, self.ref_normal = (self.xyz, self.normal) if gt is None else gt.torch_attr()[:2]
         self.enc_svh = SparseFeatureHierarchy(voxel_size, depth, dev).build_point_splatting(self.xyz)
         self.gt_svh = SparseFeatureHierarchy(voxel_size, depth, dev).build_adaptive_normal_variation(
-            self.xyz, self.normal, adaptive_depth=adaptive_depth)
+            self.ref_xyz, self.ref_normal, adaptive_depth=adaptive_depth)
         self.adaptive_depth = adaptive_depth
 
 
@@ -179,13 +188,39 @@ def gt_surface_loss(field, ref_xyz, ref_normal, subsample=GT_SURFACE_SUBSAMPLE, 
     return ev.value.abs().mean(), 1.0 - torch.sum(g * ref_normal[idx], dim=-1).mean()
 
 
-def spatial_loss(field, ref_xyz, ref_normal, voxel_size, samplers=SPATIAL_SAMPLERS, gt_band=GT_BAND, generator=None):
+def spatial_loss(field, ref_xyz, ref_normal, voxel_size, samplers=SPATIAL_SAMPLERS, gt_band=GT_BAND, generator=None,
+                 gt=None):
     """near-surface L1 of the transformed field against the transformed point-cloud SDF, / voxel_size, over the uniform +
-    band samples (models/loss.py:201-260).  Without GT geometry every sample counts as near-surface."""
+    band samples (models/loss.py:201-260).  Without GT geometry every sample counts as near-surface; with `gt` (a
+    PointTSDFVolume) the loss is spatial_volume_terms' near + empty sums over the number of samples."""
+    if gt is not None:
+        near, empty, n = spatial_volume_terms(field, ref_xyz, ref_normal, voxel_size, gt, samplers, gt_band, generator)
+        return (near + empty) / n
     q = udf_samples(field.svh, ref_xyz, ref_normal, voxel_size, samplers, generator)
     gt = transform_field(-sdf_from_points(q, ref_xyz, ref_normal, 8, 0.02, False)[0], voxel_size, gt_band)
     pd = transform_field(field.evaluate_f(q).value, voxel_size, gt_band)
     return torch.sum(torch.abs((pd - gt) / voxel_size)) / q.shape[0]
+
+
+EMPTY_SPACE_WEIGHT = 0.1     # models/loss.py:244-245: 0.1 exp(pd / (2 voxel_size)) on empty-space samples
+
+
+def spatial_volume_terms(field, ref_xyz, ref_normal, voxel_size, gt, samplers=SPATIAL_SAMPLERS, gt_band=GT_BAND,
+                         generator=None):
+    """the spatial loss's two sums with volume ground truth (models/loss.py:227-248) and the number of samples:
+    near = sum over the near-surface samples (class 0 of gt.query_classification) of |transform(pd) -
+    transform(gt.query_sdf(q))| / voxel_size; empty = sum over the empty-space samples (class 1) of
+    0.1 exp(pd / (2 voxel_size)) of the raw prediction, which pushes the field down in observed free space.  Unknown
+    samples (class 2) get neither term."""
+    q = udf_samples(field.svh, ref_xyz, ref_normal, voxel_size, samplers, generator)
+    pd = field.evaluate_f(q).value
+    gt_tsdf = transform_field(gt.query_sdf(q), voxel_size, gt_band)
+    cls = gt.query_classification(q)
+    near, empty = cls == 0, cls == 1
+    pd_tsdf = transform_field(pd, voxel_size, gt_band)
+    l_near = torch.sum(torch.abs((pd_tsdf[near] - gt_tsdf[near]) / voxel_size))
+    l_empty = torch.sum(EMPTY_SPACE_WEIGHT * torch.exp(pd[empty] / (2.0 * voxel_size)))
+    return l_near, l_empty, q.shape[0]
 
 
 def neural_field(net, feat, dec_svh: SparseFeatureHierarchy):
@@ -198,7 +233,8 @@ def neural_field(net, feat, dec_svh: SparseFeatureHierarchy):
 def kernel_losses(net, scene: TrainingScene, generator=None, feat=None, dec_svh=None, timer=None):
     """the field losses of a trainable NKSRNetwork on the scene: dict(total, gt_value, gt_normal, spatial, field), on
     the KernelField (kernel_field), or with geometry='neural' on the NeuralField (neural_field, no solve).  `feat`,
-    `dec_svh`: an existing forward of the network (else one is run)."""
+    `dec_svh`: an existing forward of the network (else one is run).  With volume ground truth (scene.gt) the dict
+    also holds spatial_empty, the empty-space term's share of spatial."""
     if feat is None:
         enc = net.encoder(scene.xyz, scene.normal, scene.enc_svh, 0)
         feat, dec_svh, _ = net.unet(enc, scene.enc_svh, adaptive_depth=scene.adaptive_depth)
@@ -206,10 +242,17 @@ def kernel_losses(net, scene: TrainingScene, generator=None, feat=None, dec_svh=
         field = neural_field(net, feat, dec_svh)
     else:
         field = kernel_field(net, feat, dec_svh, scene, timer)
-    l_val, l_nrm = gt_surface_loss(field, scene.xyz, scene.normal, generator=generator)
-    l_sp = spatial_loss(field, scene.xyz, scene.normal, scene.voxel_size, generator=generator)
+    l_val, l_nrm = gt_surface_loss(field, scene.ref_xyz, scene.ref_normal, generator=generator)
+    extra = {}
+    if scene.gt is None:
+        l_sp = spatial_loss(field, scene.xyz, scene.normal, scene.voxel_size, generator=generator)
+    else:
+        near, empty, n = spatial_volume_terms(field, scene.ref_xyz, scene.ref_normal, scene.voxel_size, scene.gt,
+                                              generator=generator)
+        l_sp = (near + empty) / n
+        extra["spatial_empty"] = empty / n
     total = GT_SURFACE_VALUE_WEIGHT * l_val + GT_SURFACE_NORMAL_WEIGHT * l_nrm + SPATIAL_WEIGHT * l_sp
-    return dict(total=total, gt_value=l_val, gt_normal=l_nrm, spatial=l_sp, field=field)
+    return dict(total=total, gt_value=l_val, gt_normal=l_nrm, spatial=l_sp, **extra, field=field)
 
 
 def use_predicted_structure(pd_structure_prob, generator=None):
@@ -241,8 +284,8 @@ def losses(net, scene: TrainingScene, generator=None, kernel=False, timer=None, 
         feat, dec_svh, udf_svh = net.unet(enc, scene.enc_svh, adaptive_depth=scene.adaptive_depth)
     l_struct, _ = structure_loss(feat.structure_features, udf_svh, scene.gt_svh)
     loss_fn = udf_field_loss if getattr(net, "udf_enabled", False) else udf_loss
-    l_udf = loss_fn(net.udf_decoder, feat.udf_features, udf_svh, scene.xyz, scene.normal, scene.voxel_size,
-                    generator=generator)
+    l_udf = loss_fn(net.udf_decoder, feat.udf_features, udf_svh, scene.ref_xyz, scene.ref_normal, scene.voxel_size,
+                    generator=generator, gt=scene.gt)
     total = STRUCTURE_WEIGHT * l_struct + UDF_WEIGHT * l_udf
     if not kernel:
         return total, l_struct, l_udf

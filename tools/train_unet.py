@@ -7,6 +7,7 @@ the structure and UDF losses (nksr_b200/training.py), Adam lr 1e-4, gradient nor
     python tools/train_unet.py --scene cfg4 --points 1000000 --depth 4 --structure predicted --steps 10
     python tools/train_unet.py --scene cfg4 --points 1000000 --depth 4 --udf --steps 10
     python tools/train_unet.py --scene sphere --points 200000 --depth 4 --geometry neural --steps 30
+    python tools/train_unet.py --scene cfg4 --points 1000000 --depth 4 --kernel-losses --vol-sup --steps 10
 
 Scenes: 'sphere' (tests/clouds.py, exact normals) or 'cfg4' (a crop of bench.py's outdoor scene at its own density,
 normals from the kNN preprocess).  Every step prints one JSON line: the losses and the CUDA-event times of the forward,
@@ -24,6 +25,11 @@ step and the backbone's forward time on the encoder hierarchy against the grown 
 output field sdf_decoder(u(x)), whose normal loss trains through its position gradient (no solve).
 --udf builds the network with udf.enabled: the UDF loss is the NeuralField's over every level of the decoder hierarchy,
 through the interpolation kernels (csrc/neural_field.cu), instead of the finest level's alone.
+--vol-sup (cfg4 only) trains with volume ground truth, the reference's default supervision: a PointTSDFVolume built from
+the crop's sensor rays (csrc/tsdf_volume.cu, DESIGN.md SPEC S19) with node spacing h = W, truncation tau = 2 W and a
+margin of one top-level voxel around the points -- our choices, the reference ships its volumes as data.  The setup
+line reports the build time and the near / free / unknown fractions of the nodes; with --kernel-losses every step
+reports the spatial loss's empty-space term (spatial_empty).
 --out saves {'state_dict': ...}, which load_checkpoint_from_url(<path>) + load_state_dict take."""
 import argparse
 import json
@@ -37,7 +43,29 @@ if ROOT not in sys.path:
 os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")
 
 
-def make_scene(kind, n, depth, device):
+def cfg4_crop(n, device):
+    """points, normals and sensor positions of an n-point cfg4 crop after get_estimate_normal_preprocess_fn(64, 85.0)
+    (kNN normals, grazing-angle filter), and the voxel size"""
+    import torch
+    from nksr_b200 import _lib
+    from nksr_b200.reconstructor import estimate_normals_knn
+    from tests import scenes
+    xyz, sensor, W = scenes.crop("cfg4_outdoor", n, with_sensor=True)
+    r = estimate_normals_knn(torch.from_numpy(xyz).to(device), torch.from_numpy(sensor).to(device), 64, 85.0)
+    scan = _lib.exclusive_scan32(r.keep)
+    cnt = int(scan[-1].item())
+    px, pn, ps = (_lib.compact_rows(a, r.keep, scan, cnt) for a in (r.xyz, r.normal, r.sensor))
+    return px, pn, ps, W
+
+
+def build_volume(px, pn, ps, W, depth):
+    """the volume ground truth of --vol-sup: h = W, tau = 2 W, a margin of one top-level voxel"""
+    from nksr_b200.gt_geometry import PointTSDFVolume
+    return PointTSDFVolume.from_sensor_rays(px, pn, ps, h=W, tau=2.0 * W, margin=W * 2 ** (depth - 1))
+
+
+def make_scene(kind, n, depth, device, vol_sup=False):
+    """the TrainingScene, and with vol_sup the volume's grid, build time (ms) and class fractions"""
     import numpy as np
     import torch
     from nksr_b200.training import TrainingScene
@@ -45,12 +73,18 @@ def make_scene(kind, n, depth, device):
     if kind == "sphere":
         from tests import clouds
         xyz, nrm = clouds.sphere(n, noise=0.001)
-        return TrainingScene(t(xyz), t(nrm), 0.02 if n <= 300_000 else 0.01, depth)
-    import nksr_b200
-    from tests import scenes
-    xyz, sensor, W = scenes.crop("cfg4_outdoor", n, with_sensor=True)
-    px, pn, _ = nksr_b200.get_estimate_normal_preprocess_fn(64, 85.0)(t(xyz), None, t(sensor))
-    return TrainingScene(px, pn, W, depth)
+        return TrainingScene(t(xyz), t(nrm), 0.02 if n <= 300_000 else 0.01, depth), None
+    px, pn, ps, W = cfg4_crop(n, device)
+    if not vol_sup:
+        return TrainingScene(px, pn, W, depth), None
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    gt = build_volume(px, pn, ps, W, depth)
+    e1.record()
+    torch.cuda.synchronize()
+    vol = dict(dims=list(gt.volume.shape), build_ms=round(e0.elapsed_time(e1), 3),
+               fractions={k: round(v, 5) for k, v in gt.class_fractions().items()})
+    return TrainingScene(px, pn, W, depth, gt=gt), vol
 
 
 class KernelTimer:
@@ -166,6 +200,8 @@ def main(argv=None):
                     help="--structure predicted: probability of growing from the prediction instead of teacher forcing")
     ap.add_argument("--udf", action="store_true",
                     help="udf.enabled: the UDF loss on the NeuralField over every level (DESIGN.md SPEC S17)")
+    ap.add_argument("--vol-sup", action="store_true",
+                    help="cfg4: volume ground truth from the sensor rays (DESIGN.md SPEC S19)")
     ap.add_argument("--geometry", choices=("kernel", "neural"), default="kernel",
                     help="output field: the kernel solve, or the NeuralField sdf_decoder(u(x)) (implies --kernel-losses)")
     args = ap.parse_args(argv)
@@ -173,6 +209,8 @@ def main(argv=None):
         args.kernel_losses = True
     if args.steps < 1:
         ap.error("--steps must be >= 1")
+    if args.vol_sup and args.scene != "cfg4":
+        ap.error("--vol-sup needs --scene cfg4 (its points carry their sensor positions)")
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("train_unet.py needs a CUDA device")
@@ -183,7 +221,7 @@ def main(argv=None):
     from nksr_b200.network import NKSRNetwork
     torch.use_deterministic_algorithms(True, warn_only=True)
     dev = torch.device("cuda:0")
-    scene = make_scene(args.scene, args.points, args.depth, dev)
+    scene, vol = make_scene(args.scene, args.points, args.depth, dev, args.vol_sup)
     net = NKSRNetwork(dict(backbone="unet", tree_depth=args.depth, kernel_dim=4, precision=args.precision,
                            trainable=True, seed=args.seed, structure=args.structure,
                            udf=dict(enabled=args.udf), geometry=args.geometry)).to(dev)
@@ -194,6 +232,8 @@ def main(argv=None):
                 depth=args.depth, precision=args.precision, structure=args.structure,
                 pd_structure_prob=args.pd_structure_prob, udf=args.udf, geometry=args.geometry,
                 voxels=[scene.enc_svh.num_voxels(l) for l in range(args.depth)])
+    if vol is not None:
+        info["volume"] = vol
     print(json.dumps(dict(setup=info)), flush=True)
     rows = []
     for step in range(args.steps):
