@@ -299,19 +299,23 @@ NKSR_API int nksr_spmv_stream_planned(const int64_t* rowptr, const int32_t* col,
 NKSR_API size_t nksr_op_workspace_bytes(const nksr_svh_t* svh, const nksr_constraints_t* c, int item_size);
 /* once per system: merges the two location orders, cuts the work items (item_size >= 1: at most that many locations,
  * cut only between voxels of levels <= 2, never across a top-level voxel; one such voxel with more locations is an
- * item of its own), then rhs b = E^T W t and the Jacobi diagonal diag(A) */
+ * item of its own), then rhs b = E^T W t and the Jacobi diagonal diag(A).  owned (nullable, one byte per unknown,
+ * levels concatenated): keep only the locations that have, on some level, an owned unknown among the 27 neighbours of
+ * their containing voxel, in the same order.  Rows i with owned[i] != 0 then get the rhs, diagonal and A x of the
+ * whole system; the other rows are incomplete.  NULL keeps every location. */
 NKSR_API int nksr_op_setup(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
                            const int32_t* base_pos, const int32_t* base_nrm, const int64_t* key_pos,
-                           const int64_t* key_nrm, int item_size, float* rhs, float* diag, void* ws, size_t ws_bytes,
-                           void* stream);
+                           const int64_t* key_nrm, const uint8_t* owned, int item_size, float* rhs, float* diag,
+                           void* ws, size_t ws_bytes, void* stream);
 /* y = A x over a workspace that nksr_op_setup prepared for the same hierarchy, features and constraints.  No atomics:
  * the same x gives bitwise the same y */
 NKSR_API int nksr_op_apply(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
                            const int32_t* base_pos, const int32_t* base_nrm, const float* x, float* y, void* ws,
                            size_t ws_bytes, void* stream);
-/* out[4] (host) = byte offsets in a workspace of ws_bytes bytes of the merged location order ([m] int32: r >= 0 position
- * r, ~r normal location r), its containing voxels ([depth][m] int32), the item count (int32) and the items ([count]
- * int4: begin, end, flags 1 first / 2 last item of its top-level voxel, 0) */
+/* out[5] (host) = byte offsets in a workspace of ws_bytes bytes of the merged location order ([m] int32: r >= 0 position
+ * r, ~r normal location r; its first `kept` entries are used), its containing voxels ([depth][m] int32), the item
+ * count (int32), the items ([count] int4: begin, end, flags 1 first / 2 last item of its top-level voxel, 0) and the
+ * kept location count (int32: m without the owned filter) */
 NKSR_API int nksr_op_workspace_layout(const nksr_svh_t* svh, const nksr_constraints_t* c, size_t ws_bytes,
                                       int64_t* out);
 /* nksr_pcg_solve with the matrix-free A: op_ws prepared by nksr_op_setup (which gave diag and b), ws of
@@ -335,6 +339,13 @@ NKSR_API int nksr_dcg_begin(void* ws, const double* red, float tol, int max_iter
 /* w = A u on owned rows, red = local {(r,u), (w,u), (r,r)}; no-op once the solve is over */
 NKSR_API int nksr_dcg_spmv_dots(const int64_t* rowptr, const int32_t* col, const float* val, const uint8_t* owned,
                        const float* r, const float* u, float* w, int64_t n, void* ws, double* red, void* stream);
+/* nksr_dcg_spmv_dots with the matrix-free A of a workspace that nksr_op_setup prepared (with the same owned mask, or
+ * NULL): w = A u on owned rows (the arithmetic of nksr_op_apply), w = 0 on the others, red = local {(r,u), (w,u),
+ * (r,r)} over the owned rows; n = the hierarchy's unknowns.  No-op once the solve is over */
+NKSR_API int nksr_dcg_op_dots(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
+                              const int32_t* base_pos, const int32_t* base_nrm, void* op_ws, size_t op_ws_bytes,
+                              const uint8_t* owned, const float* r, const float* u, float* w, void* ws, double* red,
+                              void* stream);
 /* red = all-reduced sums: convergence verdict on the device, else p,s,x,r,u advance one iteration */
 NKSR_API int nksr_dcg_update(const float* diag, const uint8_t* owned, float* x, float* r, float* u, const float* w,
                     float* p, float* s, int64_t n, void* ws, const double* red, void* stream);

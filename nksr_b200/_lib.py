@@ -97,7 +97,7 @@ _SIGNATURES = {
     "nksr_spmv_plan_stats": ("i", "ppp"),
     "nksr_spmv_stream_planned": ("i", "ppppp" + "qqqq" + "pp"),
     "nksr_op_workspace_bytes": ("z", "SKi"),
-    "nksr_op_setup": ("i", "SFK" + "ppppi" + "pppzp"),
+    "nksr_op_setup": ("i", "SFK" + "pppppi" + "pppzp"),
     "nksr_op_apply": ("i", "SFK" + "pppppzp"),
     "nksr_op_workspace_layout": ("i", "SKzp"),
     "nksr_pcg_solve_matrix_free": ("i", "SFK" + "ppppp" + "fiii" + "pzpzdp"),
@@ -105,6 +105,7 @@ _SIGNATURES = {
     "nksr_dcg_init": ("i", "pppppppp" + "q" + "pz" + "pp"),
     "nksr_dcg_begin": ("i", "ppfip"),
     "nksr_dcg_spmv_dots": ("i", "ppppppp" + "q" + "ppp"),
+    "nksr_dcg_op_dots": ("i", "SFK" + "pppz" + "pppp" + "ppp"),
     "nksr_dcg_update": ("i", "pppppppp" + "q" + "ppp"),
     "nksr_dcg_status": ("i", "pdp"),
     "nksr_gather_f32": ("i", "ppqpp"),

@@ -61,13 +61,37 @@ __device__ __forceinline__ EdgeBuffers op_edge_buffers(const MfOperator& op) {
 }
 
 // ------------------------------------------------------------------------------------------------- setup: the items
-// merged position of every location: positions first on equal keys (a stable merge of the two sorted key lists)
+// owned-location filter: keep[i] = 1 when location i (positions, then normal locations) has, on some level l, an owned
+// unknown among the 27 neighbours of its containing voxel -- the only rows it contributes to.  One warp per location,
+// lane = stencil slot
+__global__ void k_op_keep(nksr_svh_t svh, const int32_t* __restrict__ bp, int64_t np, const int32_t* __restrict__ bn,
+                          int64_t nn, const uint8_t* __restrict__ owned, int32_t* __restrict__ keep) {
+  const int lane = threadIdx.x & 31;
+  const int64_t i = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+  if (i >= np + nn) return;
+  const bool pos = i < np;
+  const int32_t* b = pos ? bp + i : bn + (i - np);
+  const int64_t nb = pos ? np : nn;
+  bool any = false;
+  for (int l = 0; l < svh.depth && !any; ++l) {
+    const int v = __ldg(b + l * nb);
+    if (v < 0) continue;
+    const int u = lane < 27 ? __ldg(svh.nbr27[l] + (int64_t)v * 27 + lane) : -1;
+    any = __any_sync(0xffffffffu, u >= 0 && __ldg(owned + svh.offset[l] + u) != 0);
+  }
+  if (lane == 0) keep[i] = any ? 1 : 0;
+}
+
+// merged position of every location: positions first on equal keys (a stable merge of the two sorted key lists).
+// keep != nullptr: the exclusive scan of the filter's flags over m + 1 entries; only the kept locations are merged, to
+// the first keep[m] slots, in the same relative order
 __global__ void k_op_merge(const int64_t* __restrict__ kp, int64_t np, const int64_t* __restrict__ kn, int64_t nn,
                            const int32_t* __restrict__ bp, const int32_t* __restrict__ bn, int L,
-                           int32_t* __restrict__ seq, int32_t* __restrict__ vox) {
+                           const int32_t* __restrict__ keep, int32_t* __restrict__ seq, int32_t* __restrict__ vox) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   const int64_t m = np + nn;
   if (i >= m) return;
+  if (keep && keep[i + 1] == keep[i]) return;
   const bool pos = i < np;
   const int64_t r = pos ? i : i - np;
   const int64_t key = pos ? kp[r] : kn[r];
@@ -78,7 +102,9 @@ __global__ void k_op_merge(const int64_t* __restrict__ kp, int64_t np, const int
     const int64_t v = __ldg(other + mid);
     if (pos ? v < key : v <= key) lo = mid + 1; else hi = mid;
   }
-  const int64_t rank = r + lo;
+  // the same count over the kept locations only: kept ones of my kind before me plus kept ones of the other before me
+  const int64_t rank = !keep ? r + lo
+                     : pos ? keep[i] + (keep[np + lo] - keep[np]) : (keep[i] - keep[np]) + keep[lo];
   seq[rank] = pos ? (int32_t)r : ~(int32_t)r;
   const int32_t* b = pos ? bp : bn;
   const int64_t nb = pos ? np : nn;
@@ -404,7 +430,50 @@ __global__ void __launch_bounds__(kEdgeBlock) k_op_edges(MfOperator op, const in
   }
 }
 
-// y = sum_s P[s][nbr27(i)[26 - s]] + w_reg R x (SETUP: y = rhs from P, y2 = diag from Pd + w_reg R_ii)
+// row g of y = sum_s P[s][nbr27(i)[26 - s]] + w_reg R x (SETUP: y = rhs from P, y2 = diag from Pd + w_reg R_ii)
+template <bool SETUP>
+__device__ __forceinline__ void op_apply_row(const nksr_svh_t& svh, const nksr_feat_t& feat, float w_reg,
+                                             const float* __restrict__ P, const float* __restrict__ Pd,
+                                             const float* __restrict__ x, int64_t n, int64_t g, float& y, float& y2) {
+  const int C = feat.channels;
+  // the level of g: the last one that starts at or before g (an empty level starts where the next one does).
+  // Unrolled, so that the level's pointers come from the parameter space, not a local copy of the struct
+  int64_t off = 0;
+  const int32_t* nbt = svh.nbr27[0];
+  const float* zt = feat.z[0];
+#pragma unroll
+  for (int k = 1; k < NKSR_MAX_DEPTH; ++k)
+    if (k < svh.depth && g >= svh.offset[k]) { off = svh.offset[k]; nbt = svh.nbr27[k]; zt = feat.z[k]; }
+  const int64_t i = g - off;
+  const int32_t* nb = nbt + i * 27;
+  const float* zi = zt + i * C;
+  float s = 0.f, sd = 0.f, reg = 0.f;
+#pragma unroll 3
+  for (int k = 0; k < 27; ++k) {
+    const int v = __ldg(nb + k);
+    if (v < 0) continue;
+    const int64_t q = (int64_t)(26 - k) * n + off + v;
+    s += __ldg(P + q);
+    if (SETUP) sd += __ldg(Pd + q);
+    if (w_reg != 0.f && (!SETUP || k == 13)) {
+      const float* zn = zt + (int64_t)v * C;
+      float d = 0.f;
+      for (int c = 0; c < C; ++c) d = fmaf(__ldg(zi + c), __ldg(zn + c), d);
+      const int dx = k / 9 - 1, dy = (k / 3) % 3 - 1, dz = k % 3 - 1;
+      const float bw = (dx == 0 ? 0.75f : 0.125f) * (dy == 0 ? 0.75f : 0.125f) * (dz == 0 ? 0.75f : 0.125f);
+      if (SETUP) sd += w_reg * bw * d;
+      else reg = fmaf(w_reg * bw * d, __ldg(x + off + v), reg);
+    }
+  }
+  if (SETUP) {
+    y = s;
+    y2 = sd;
+  } else {
+    y = s + reg;
+  }
+}
+
+// one thread per unknown, grid-stride: y (and y2) of op_apply_row; pap != nullptr: pap[b] = block b's sum of x_i y_i
 template <bool SETUP>
 __global__ void __launch_bounds__(kApplyBlock)
 k_op_apply(nksr_svh_t svh, nksr_feat_t feat, float w_reg, const float* __restrict__ P, const float* __restrict__ Pd,
@@ -412,46 +481,13 @@ k_op_apply(nksr_svh_t svh, nksr_feat_t feat, float w_reg, const float* __restric
            double* __restrict__ pap, const int* __restrict__ done) {
   __shared__ double sh[kApplyBlock / 32];
   if (done && *done) return;
-  const int C = feat.channels;
   double local = 0.0;
   for (int64_t g = blockIdx.x * (int64_t)kApplyBlock + threadIdx.x; g < n; g += (int64_t)gridDim.x * kApplyBlock) {
-    // the level of g: the last one that starts at or before g (an empty level starts where the next one does).
-    // Unrolled, so that the level's pointers come from the parameter space, not a local copy of the struct
-    int64_t off = 0;
-    const int32_t* nbt = svh.nbr27[0];
-    const float* zt = feat.z[0];
-#pragma unroll
-    for (int k = 1; k < NKSR_MAX_DEPTH; ++k)
-      if (k < svh.depth && g >= svh.offset[k]) { off = svh.offset[k]; nbt = svh.nbr27[k]; zt = feat.z[k]; }
-    const int64_t i = g - off;
-    const int32_t* nb = nbt + i * 27;
-    const float* zi = zt + i * C;
-    float s = 0.f, sd = 0.f, reg = 0.f;
-#pragma unroll 3
-    for (int k = 0; k < 27; ++k) {
-      const int v = __ldg(nb + k);
-      if (v < 0) continue;
-      const int64_t q = (int64_t)(26 - k) * n + off + v;
-      s += __ldg(P + q);
-      if (SETUP) sd += __ldg(Pd + q);
-      if (w_reg != 0.f && (!SETUP || k == 13)) {
-        const float* zn = zt + (int64_t)v * C;
-        float d = 0.f;
-        for (int c = 0; c < C; ++c) d = fmaf(__ldg(zi + c), __ldg(zn + c), d);
-        const int dx = k / 9 - 1, dy = (k / 3) % 3 - 1, dz = k % 3 - 1;
-        const float bw = (dx == 0 ? 0.75f : 0.125f) * (dy == 0 ? 0.75f : 0.125f) * (dz == 0 ? 0.75f : 0.125f);
-        if (SETUP) sd += w_reg * bw * d;
-        else reg = fmaf(w_reg * bw * d, __ldg(x + off + v), reg);
-      }
-    }
-    if (SETUP) {
-      y[g] = s;
-      y2[g] = sd;
-    } else {
-      const float yi = s + reg;
-      y[g] = yi;
-      if (pap) local += (double)yi * (double)__ldg(x + g);
-    }
+    float yi, y2i;
+    op_apply_row<SETUP>(svh, feat, w_reg, P, Pd, x, n, g, yi, y2i);
+    y[g] = yi;
+    if (SETUP) y2[g] = y2i;
+    else if (pap) local += (double)yi * (double)__ldg(x + g);
   }
   if (pap) {
     local = warp_sum_d(local);
@@ -465,6 +501,45 @@ k_op_apply(nksr_svh_t svh, nksr_feat_t feat, float w_reg, const float* __restric
   }
 }
 
+// the distributed solve's step (x = u): w = A u on the rows with owned[g] != 0 (op_apply_row, the arithmetic of
+// k_op_apply) and 0 on the others; dots[j * gridDim.x + block] = the block's sums over the owned rows of (r,u), (w,u),
+// (r,r) for j = 0, 1, 2.  (4 blocks per SM caps it at 64 registers: without the cap ptxas held it at 40 and spilled
+// the three accumulators)
+__global__ void __launch_bounds__(kApplyBlock, 4)
+k_op_apply_dcg(nksr_svh_t svh, nksr_feat_t feat, float w_reg, const float* __restrict__ P,
+               const uint8_t* __restrict__ owned, const float* __restrict__ r, const float* __restrict__ u,
+               float* __restrict__ w, int64_t n, double* __restrict__ dots, const int* __restrict__ done) {
+  __shared__ double sh[3][kApplyBlock / 32];
+  if (*done) return;
+  double ru = 0.0, wu = 0.0, rr = 0.0;
+  for (int64_t g = blockIdx.x * (int64_t)kApplyBlock + threadIdx.x; g < n; g += (int64_t)gridDim.x * kApplyBlock) {
+    if (!__ldg(owned + g)) {
+      w[g] = 0.f;
+      continue;
+    }
+    float wi, unused;
+    op_apply_row<false>(svh, feat, w_reg, P, nullptr, u, n, g, wi, unused);
+    w[g] = wi;
+    const double ri = (double)__ldg(r + g), ui = (double)__ldg(u + g);
+    ru += ri * ui;
+    wu += (double)wi * ui;
+    rr += ri * ri;
+  }
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  ru = warp_sum_d(ru);
+  wu = warp_sum_d(wu);
+  rr = warp_sum_d(rr);
+  if (lane == 0) { sh[0][wid] = ru; sh[1][wid] = wu; sh[2][wid] = rr; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t0 = 0.0, t1 = 0.0, t2 = 0.0;
+    for (int k = 0; k < kApplyBlock / 32; ++k) { t0 += sh[0][k]; t1 += sh[1][k]; t2 += sh[2][k]; }
+    dots[blockIdx.x] = t0;
+    dots[gridDim.x + blockIdx.x] = t1;
+    dots[2 * gridDim.x + blockIdx.x] = t2;
+  }
+}
+
 // -------------------------------------------------------------------------------------------------------- host side
 size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
@@ -475,19 +550,22 @@ int edge_levels(const nksr_svh_t& svh) {
   return svh.depth - 1 - cut;
 }
 
-// workspace: P, Pd, the merged sequence and its voxels, top ranges, item counts and offsets, the item count, the scan's
-// scratch (the fixed part), then as many items with their edge slots as the rest holds
+// workspace: P, Pd, the merged sequence and its voxels, top ranges, item counts and offsets, the item count, the
+// owned-location filter's flags and the kept count, the scans' scratch (the fixed part), then as many items with their
+// edge slots as the rest holds
 struct OpLayout {
-  size_t P, Pd, seq, vox, top, cnt, ofs, n_items, max_items, scan, scan_bytes, fixed;
+  size_t P, Pd, seq, vox, top, cnt, ofs, n_items, max_items, keep, n_kept, scan, scan_bytes, fixed;
   size_t per_item;   // item record + its edge slots (rhs and diagonal)
 };
 
 OpLayout op_layout(const nksr_svh_t& svh, int64_t m) {
   OpLayout o;
   const int64_t n = op_unknowns(svh), n_top = svh.n[svh.depth - 1];
-  o.scan_bytes = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, o.scan_bytes, (const int32_t*)nullptr, (int32_t*)nullptr,
+  size_t top_scan = 0, keep_scan = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, top_scan, (const int32_t*)nullptr, (int32_t*)nullptr,
                                 (int)(n_top > 0 ? n_top : 1));
+  cub::DeviceScan::ExclusiveSum(nullptr, keep_scan, (const int32_t*)nullptr, (int32_t*)nullptr, (int)(m + 1));
+  o.scan_bytes = top_scan > keep_scan ? top_scan : keep_scan;
   size_t at = 0;
   auto take = [&](size_t bytes) { const size_t p = at; at += align256(bytes); return p; };
   o.P = take((size_t)27 * n * sizeof(float));
@@ -499,6 +577,8 @@ OpLayout op_layout(const nksr_svh_t& svh, int64_t m) {
   o.ofs = take((size_t)n_top * sizeof(int32_t));
   o.n_items = take(sizeof(int32_t));
   o.max_items = take(sizeof(int64_t));
+  o.keep = take((size_t)(m + 1) * sizeof(int32_t));
+  o.n_kept = take(sizeof(int32_t));
   o.scan = take(o.scan_bytes);
   o.fixed = at;
   o.per_item = sizeof(int4) + 2 * (size_t)edge_levels(svh) * 2 * 27 * sizeof(float);
@@ -609,6 +689,13 @@ int mf_apply_launch(const MfOperator& op, const float* x, float* y, double* pap,
   return NKSR_OK;
 }
 
+int mf_dcg_launch(const MfOperator& op, const uint8_t* owned, const float* r, const float* u, float* w, double* dots,
+                  int blocks, const int* done, cudaStream_t s) {
+  walk_launch<false>(op, u, done, s);
+  k_op_apply_dcg<<<blocks, kApplyBlock, 0, s>>>(op.svh, op.feat, op.cs.w_reg, op.P, owned, r, u, w, op.n, dots, done);
+  return NKSR_OK;
+}
+
 extern "C" {
 
 size_t nksr_op_workspace_bytes(const nksr_svh_t* svh, const nksr_constraints_t* c, int item_size) {
@@ -618,8 +705,8 @@ size_t nksr_op_workspace_bytes(const nksr_svh_t* svh, const nksr_constraints_t* 
 }
 
 int nksr_op_setup(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c, const int32_t* base_pos,
-                  const int32_t* base_nrm, const int64_t* key_pos, const int64_t* key_nrm, int item_size, float* rhs,
-                  float* diag, void* ws, size_t ws_bytes, void* stream) {
+                  const int32_t* base_nrm, const int64_t* key_pos, const int64_t* key_nrm, const uint8_t* owned,
+                  int item_size, float* rhs, float* diag, void* ws, size_t ws_bytes, void* stream) {
   if (!op_valid(svh, feat, c, base_pos, base_nrm) || !rhs || !diag || !ws || item_size < 1) return NKSR_E_INVALID;
   if ((c->n_pos > 0 && !key_pos) || (c->n_nrm > 0 && !key_nrm)) return NKSR_E_INVALID;
   const int64_t m = c->n_pos + c->n_nrm;
@@ -634,10 +721,27 @@ int nksr_op_setup(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_con
   if (cudaMemsetAsync(ws, 0, o.fixed, s) != cudaSuccess) return NKSR_E_CUDA;
   if (cudaMemcpyAsync(op.max_items, &max_items, sizeof(int64_t), cudaMemcpyHostToDevice, s) != cudaSuccess)
     return NKSR_E_CUDA;
+  unsigned char* w = reinterpret_cast<unsigned char*>(ws);
+  int32_t* keep = reinterpret_cast<int32_t*>(w + o.keep);
+  int32_t* n_kept = reinterpret_cast<int32_t*>(w + o.n_kept);
+  const int32_t m32 = (int32_t)m;
+  if (!owned && cudaMemcpyAsync(n_kept, &m32, sizeof(int32_t), cudaMemcpyHostToDevice, s) != cudaSuccess)
+    return NKSR_E_CUDA;
   const int64_t n_top = svh->n[svh->depth - 1];
   if (m > 0 && n_top > 0) {
+    if (owned) {
+      // the filter: flags, their exclusive scan in place over m + 1 entries (keep[m] = 0 from the clear, so keep[m]
+      // becomes the kept count), and the vox entries past the kept ones read as "no voxel"
+      k_op_keep<<<grid_for(m * 32, 256), 256, 0, s>>>(*svh, base_pos, c->n_pos, base_nrm, c->n_nrm, owned, keep);
+      size_t kb = op.scan_bytes;
+      if (cub::DeviceScan::ExclusiveSum(op.scan_tmp, kb, keep, keep, (int)(m + 1), s) != cudaSuccess)
+        return NKSR_E_CUDA;
+      if (cudaMemcpyAsync(n_kept, keep + m, sizeof(int32_t), cudaMemcpyDeviceToDevice, s) != cudaSuccess ||
+          cudaMemsetAsync(op.vox, 0xff, (size_t)svh->depth * m * sizeof(int32_t), s) != cudaSuccess)
+        return NKSR_E_CUDA;
+    }
     k_op_merge<<<grid_for(m, 256), 256, 0, s>>>(key_pos, c->n_pos, key_nrm, c->n_nrm, base_pos, base_nrm, svh->depth,
-                                               op.seq, op.vox);
+                                               owned ? keep : nullptr, op.seq, op.vox);
     k_op_top_ranges<<<grid_for(m, 256), 256, 0, s>>>(op.vox + (int64_t)(svh->depth - 1) * m, m, op.top);
     const int cut = svh->depth - 1 < kCutLevel ? svh->depth - 1 : kCutLevel;
     const int grid = grid_for(n_top * 32, 256);
@@ -676,6 +780,7 @@ int nksr_op_workspace_layout(const nksr_svh_t* svh, const nksr_constraints_t* c,
   out[1] = (int64_t)o.vox;
   out[2] = (int64_t)o.n_items;
   out[3] = (int64_t)o.fixed;
+  out[4] = (int64_t)o.n_kept;
   return NKSR_OK;
 }
 

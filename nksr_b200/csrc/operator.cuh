@@ -39,3 +39,9 @@ int mf_operator_make(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_
 // of 256 threads (the fixed-order partials the PCG reduces).  done != nullptr: every kernel is a no-op once *done.
 int mf_apply_launch(const MfOperator& op, const float* x, float* y, double* pap, int blocks, const int* done,
                     cudaStream_t s);
+
+// the distributed solve's step: w = A u on the rows with owned[i] != 0, w = 0 on the others, and dots[j * blocks + b]
+// = block b's sums over the owned rows of (r,u), (w,u), (r,r) (j = 0, 1, 2) for a grid of exactly `blocks` blocks of
+// 256 threads.  Every kernel is a no-op once *done
+int mf_dcg_launch(const MfOperator& op, const uint8_t* owned, const float* r, const float* u, float* w, double* dots,
+                  int blocks, const int* done, cudaStream_t s);

@@ -696,6 +696,23 @@ int nksr_dcg_spmv_dots(const int64_t* rowptr, const int32_t* col, const float* v
   return NKSR_OK;
 }
 
+int nksr_dcg_op_dots(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
+                     const int32_t* base_pos, const int32_t* base_nrm, void* op_ws, size_t op_ws_bytes,
+                     const uint8_t* owned, const float* r, const float* u, float* w, void* ws, double* red,
+                     void* stream) {
+  if (!ws || !red || !owned || !r || !u || !w) return NKSR_E_INVALID;
+  MfOperator mf;
+  const int rc = mf_operator_make(svh, feat, c, base_pos, base_nrm, op_ws, op_ws_bytes, &mf);
+  if (rc != NKSR_OK) return rc;
+  cudaStream_t st = as_stream(stream);
+  DcgWs d = carve_dcg(ws);
+  // the dots land in the partial arrays of k_dcg_spmv's layout (kGrid blocks of kBlock = 256 threads)
+  mf_dcg_launch(mf, owned, r, u, w, d.part, kGrid, &d.ctrl->done, st);
+  k_reduce_arrays<<<1, kBlock, 0, st>>>(d.part, 3, red, d.ctrl);
+  NKSR_CHECK_LAUNCH();
+  return NKSR_OK;
+}
+
 int nksr_dcg_update(const float* diag, const uint8_t* owned, float* x, float* r, float* u, const float* w, float* p,
                     float* s, int64_t n, void* ws, const double* red, void* stream) {
   if (n <= 0 || !ws || !red) return NKSR_E_INVALID;

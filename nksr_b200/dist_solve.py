@@ -23,6 +23,7 @@ exchange logic is plain tensor code tested on gloo (CPU tensors).
 from __future__ import annotations
 
 import ctypes as C
+import os
 from types import SimpleNamespace
 from typing import List, Optional
 
@@ -246,7 +247,9 @@ def _gsum(t: torch.Tensor, group) -> torch.Tensor:
 def pcg_distributed(sysm, owned: torch.Tensor, plan: HaloPlan, tol: float, max_iter: int, check_every: int = 16,
                     group=None):
     """Jacobi-PCG (Chronopoulos-Gear form: one fused all-reduce per iteration) on the rows every rank owns of its
-    local CSR system.  `owned`: bool per local unknown.  Returns (x with halo entries filled, info dict)."""
+    local system: the CSR system of KernelField.assemble, or the matrix-free operator of
+    KernelField.matrix_free_system (set up with the same `owned`).  `owned`: bool per local unknown.  Returns (x with
+    halo entries filled, info dict)."""
     n, dev = sysm.n, sysm.rhs.device
     st = stream_ptr(dev)
     world = _world(group)
@@ -256,6 +259,13 @@ def pcg_distributed(sysm, owned: torch.Tensor, plan: HaloPlan, tol: float, max_i
     ws = torch.empty(nb, dtype=torch.uint8, device=dev)
     red = torch.zeros(3, dtype=torch.float64, device=dev)
     info = (C.c_double * 4)()
+    if hasattr(sysm, "rowptr"):
+        def apply_and_dots():
+            call("nksr_dcg_spmv_dots", sysm.rowptr, sysm.col, sysm.val, own8, r, u, w, n, ws, red, st)
+    else:
+        def apply_and_dots():
+            call("nksr_dcg_op_dots", sysm.svh_view, sysm.feat_view, sysm.cs, sysm.base_pos, sysm.base_nrm, sysm.ws,
+                 sysm.ws_bytes, own8, r, u, w, ws, red, st)
     call("nksr_dcg_init", sysm.diag, sysm.rhs, own8, x, r, u, p, s, n, ws, nb, red, st)
     if world > 1:
         dist.all_reduce(red, group=group)
@@ -264,7 +274,7 @@ def pcg_distributed(sysm, owned: torch.Tensor, plan: HaloPlan, tol: float, max_i
     while True:
         for _ in range(max(int(check_every), 1)):
             plan.exchange(u)
-            call("nksr_dcg_spmv_dots", sysm.rowptr, sysm.col, sysm.val, own8, r, u, w, n, ws, red, st)
+            apply_and_dots()
             if world > 1:
                 dist.all_reduce(red, group=group)
                 allreduces += 1
@@ -280,14 +290,78 @@ def pcg_distributed(sysm, owned: torch.Tensor, plan: HaloPlan, tol: float, max_i
                "iterations_launched": launched}
 
 
+def resolve_operator(operator: Optional[str] = None) -> str:
+    """The global solve's operator: the argument, else NKSR_OPERATOR, else 'assembled'."""
+    op = operator or os.environ.get("NKSR_OPERATOR") or "assembled"
+    if op not in ("matrix_free", "assembled"):
+        raise ValueError("solver_config['operator'] must be 'matrix_free' or 'assembled'")
+    return op
+
+
+def local_system(reconstructor, lx: torch.Tensor, ln: Optional[torch.Tensor], lsens: Optional[torch.Tensor],
+                 bounds: List[float], rank: int, axis: int, voxel_size: float, approx_kernel_grad: bool = False,
+                 timer=None):
+    """One rank's share of the global system, from the points routed to it (its slab [bounds[rank],
+    bounds[rank + 1]) plus halo): hierarchy, network features and KernelField of the region, the owner of every
+    unknown by voxel centre, and the constraint locations.  Touches no process group.  Returns a namespace with
+    .field, .owner (per level: owning rank of each voxel), .owned (bool per unknown), .pos_xyz, .normal_xyz,
+    .normal_value, and .counts (float64 [2]: points inside the slab, owned normal locations), which summed over the
+    ranks give the constraint weights (constraint_weights)."""
+    dev = lx.device
+    if ln is not None:
+        feat = ln
+    elif lsens is not None:
+        view = lsens - lx
+        feat = view / (torch.linalg.norm(view, dim=-1, keepdim=True) + 1e-6)
+    else:
+        raise ValueError("either normal or sensor (with a normal-estimating preprocess_fn) is required")
+    L = reconstructor.tree_depth
+    lo, hi = bounds[rank], bounds[rank + 1]
+    inside = (lx[:, axis].double() >= lo) & (lx[:, axis].double() < hi)
+    counts = torch.tensor([float(inside.sum().item()), 0.0], dtype=torch.float64, device=dev)
+
+    svh = SparseFeatureHierarchy(voxel_size, L, dev).build_point_splatting(lx)
+    net = reconstructor.network
+    enc = net.encoder(lx, feat, svh, 0)
+    feats, dec_svh, _ = net.unet(enc, svh, adaptive_depth=reconstructor.adaptive_depth)
+    field = KernelField(dec_svh, net.interpolators, feats.basis_features, approx_kernel_grad)
+    if timer is not None:
+        timer.mark("svh_and_network")
+    ad = min(reconstructor.adaptive_depth, L)
+    # ownership of every unknown / normal location by voxel-centre coordinate (exact: integer ijk)
+    owner, centres = [], []
+    for l in range(L):
+        g = SparseIndexGrid(dec_svh, l)
+        ijk = g.active_grid_coords()
+        cen = (ijk[:, axis].double() + 0.5) * (float(voxel_size) * (2 ** l))
+        owner.append(owner_of(cen, bounds))
+        centres.append(g.grid_to_world(ijk))
+    owned = torch.cat([o == rank for o in owner])
+    counts[1] = float(sum(int((owner[d] == rank).sum().item()) for d in range(ad)))
+    normal_xyz = torch.cat([centres[d] for d in range(ad)])
+    normal_value = torch.cat([feats.normal_features[d] for d in range(ad)])
+    return SimpleNamespace(field=field, owner=owner, owned=owned, pos_xyz=lx, normal_xyz=normal_xyz,
+                           normal_value=-normal_value, counts=counts, adaptive_depth=ad)
+
+
+def constraint_weights(n_points_global: float, k_global: float, voxel_size: float):
+    """(pos_weight, normal_weight, reg_weight) of the global system from the global point and normal-location counts:
+    the weights the single-GPU reconstruct uses for the whole cloud"""
+    from .reconstructor import NORMAL_WEIGHT, POS_WEIGHT
+    return POS_WEIGHT / n_points_global, NORMAL_WEIGHT / k_global * (float(voxel_size) ** 2), 1.0
+
+
 def reconstruct_global(reconstructor, xyz: torch.Tensor, normal: Optional[torch.Tensor], voxel_size: float,
                        halo_voxels: int = 8, axis: Optional[int] = None, approx_kernel_grad: bool = False,
                        solver_tol: float = 1e-5, solver_max_iter: int = 2000, group=None, sensor=None,
-                       preprocess_fn=None, distributed_input: bool = False):
+                       preprocess_fn=None, distributed_input: bool = False, operator: Optional[str] = None):
     """ONE global system over all ranks.  `distributed_input=False`: every rank passes the same whole cloud
     (each keeps its slab + halo); True: every rank passes ITS SHARE of the cloud and the points are routed to
-    the ranks that need them by one all-to-all.  Returns a KernelField over this rank's slab+halo region with
-    `.owned` (per-unknown bool), `.owned_cells` (level-0 mask for meshing) and `.solve_info`."""
+    the ranks that need them by one all-to-all.  `operator`: 'assembled' (the CSR Gram matrix of every rank's region)
+    or 'matrix_free' (A applied from the kernel rows of the locations that feed owned rows, csrc/operator.cu); None
+    reads NKSR_OPERATOR and assembles when that is unset.  Returns a KernelField over this rank's slab+halo region
+    with `.owned` (per-unknown bool), `.owned_cells` (level-0 mask for meshing) and `.solve_info`."""
+    op = resolve_operator(operator)
     if getattr(reconstructor.network, "structure", "encoder") == "predicted":
         # every rank would grow its own hierarchy from its own predictions, which can disagree in the halo
         raise _lib.NksrError("the global solve needs structure='encoder': hierarchies grown from the predicted "
@@ -337,44 +411,25 @@ def reconstruct_global(reconstructor, xyz: torch.Tensor, normal: Optional[torch.
         lx, ln, lsens = preprocess_fn(lx, ln, lsens)
         lx = lx.contiguous()
     tm.mark("preprocess")
-    if ln is not None:
-        feat = ln
-    elif lsens is not None:
-        view = lsens - lx
-        feat = view / (torch.linalg.norm(view, dim=-1, keepdim=True) + 1e-6)
-    else:
-        raise ValueError("either normal or sensor (with a normal-estimating preprocess_fn) is required")
-    inside = (lx[:, axis].double() >= lo) & (lx[:, axis].double() < hi)
-    counts = torch.tensor([float(inside.sum().item()), 0.0], dtype=torch.float64, device=dev)
-
-    svh = SparseFeatureHierarchy(voxel_size, L, dev).build_point_splatting(lx)
-    net = reconstructor.network
-    enc = net.encoder(lx, feat, svh, 0)
-    feats, dec_svh, _ = net.unet(enc, svh, adaptive_depth=reconstructor.adaptive_depth)
-    field = KernelField(dec_svh, net.interpolators, feats.basis_features, approx_kernel_grad)
-    tm.mark("svh_and_network")
-    ad = min(reconstructor.adaptive_depth, L)
-    offs = dec_svh.offsets
-    # ownership of every unknown / normal location by voxel-centre coordinate (exact: integer ijk)
-    owner, centres = [], []
-    for l in range(L):
-        g = SparseIndexGrid(dec_svh, l)
-        ijk = g.active_grid_coords()
-        cen = (ijk[:, axis].double() + 0.5) * (float(voxel_size) * (2 ** l))
-        owner.append(owner_of(cen, bounds))
-        centres.append(g.grid_to_world(ijk))
-    owned = torch.cat([o == rank for o in owner])
-    counts[1] = float(sum(int((owner[d] == rank).sum().item()) for d in range(ad)))
+    loc = local_system(reconstructor, lx, ln, lsens, bounds, rank, axis, voxel_size, approx_kernel_grad, tm)
+    field, owner, owned, counts = loc.field, loc.owner, loc.owned, loc.counts
+    dec_svh, ad = field.svh, loc.adaptive_depth
     if world > 1:
         dist.all_reduce(counts, group=group)
     n_points_global, k_global = float(counts[0].item()), float(counts[1].item())
-    normal_xyz = torch.cat([centres[d] for d in range(ad)])
-    normal_value = torch.cat([feats.normal_features[d] for d in range(ad)])
-    from .reconstructor import NORMAL_WEIGHT, POS_WEIGHT
-    sysm = field.assemble(lx, normal_xyz, -normal_value, POS_WEIGHT / n_points_global,
-                          NORMAL_WEIGHT / k_global * (float(voxel_size) ** 2), 1.0)
-    tm.mark("ownership_and_assembly")
-    plan = build_halo_plan(dec_svh.keys, owner, offs, group)
+    weights = constraint_weights(n_points_global, k_global, voxel_size)
+    if op == "matrix_free":
+        # only the locations that feed an owned row are kept: the halo's other locations cost nothing per iteration
+        sysm = field.matrix_free_system(loc.pos_xyz, loc.normal_xyz, loc.normal_value, *weights, owned=owned)
+        sysm.svh_view, sysm.feat_view = dec_svh.view(), field.feat_view()
+        tm.mark("ownership_and_operator_setup")
+        op_info = dict(operator="matrix_free", operator_bytes_per_apply=sysm.bytes_per_apply,
+                       locations_kept=sysm.locations_kept, locations_total=int(sysm.cs.n_pos + sysm.cs.n_nrm), nnz=0)
+    else:
+        sysm = field.assemble(loc.pos_xyz, loc.normal_xyz, loc.normal_value, *weights)
+        tm.mark("ownership_and_assembly")
+        op_info = dict(operator="assembled", nnz=sysm.nnz)
+    plan = build_halo_plan(dec_svh.keys, owner, dec_svh.offsets, group)
     tm.mark("halo_plan")
     alpha, info = pcg_distributed(sysm, owned, plan, solver_tol, solver_max_iter, 16, group)
     tm.mark("pcg")
@@ -382,7 +437,7 @@ def reconstruct_global(reconstructor, xyz: torch.Tensor, normal: Optional[torch.
     field.alpha = alpha
     field.owned = owned
     field.owned_cells = owner[0] == rank
-    field.solve_info = dict(info, n=sysm.n, nnz=sysm.nnz, n_owned=int(owned.sum().item()),
+    field.solve_info = dict(info, n=sysm.n, **op_info, n_owned=int(owned.sum().item()),
                             halo_recv=int(sum(plan.recv_counts)), halo_send=int(sum(plan.send_counts)),
                             halo_bytes_per_exchange=plan.bytes_per_exchange, halo_dropped=getattr(plan, "dropped", 0),
                             slab=(lo, hi), axis=axis,

@@ -284,8 +284,9 @@ class KernelField(BaseField):
         or 'assembled' (the CSR Gram matrix).  Default: matrix-free with approx_kernel_grad (compact rows) on systems of
         at least MATRIX_FREE_MIN_UNKNOWNS unknowns, assembled otherwise.  A Gram fill chosen explicitly
         (solver_config['fill'] or NKSR_FILL) asks for the matrix that fill builds, so it too selects the assembled
-        operator unless the operator is given as well.  Grad-recording solves, keep_system and the global solve always
-        assemble."""
+        operator unless the operator is given as well.  Grad-recording solves and keep_system always assemble.  The
+        global solve (dist_solve.reconstruct_global) takes the operator as an argument or from NKSR_OPERATOR, and
+        assembles when neither names one."""
         op = self.solver_config.get("operator") or os.environ.get("NKSR_OPERATOR")
         if op is None:
             big = self.svh.num_unknowns >= MATRIX_FREE_MIN_UNKNOWNS
@@ -315,11 +316,13 @@ class KernelField(BaseField):
         return alpha
 
     def matrix_free_system(self, pos_xyz, normal_xyz=None, normal_value=None, pos_weight=1.0, normal_weight=1.0,
-                           reg_weight=1.0, item_size: Optional[int] = None):
+                           reg_weight=1.0, item_size: Optional[int] = None, owned: Optional[torch.Tensor] = None):
         """Kernel rows of the sorted constraint locations and the operator's setup (nksr_op_setup): returns
-        .rhs, .diag, .n and what apply_operator needs (the rows, the constraint struct, the operator's workspace).
-        item_size: at most that many locations per work item of the gather-scatter (default OP_ITEM_SIZE; see
-        operator_items)."""
+        .rhs, .diag, .n, .locations_kept and what apply_operator needs (the rows, the constraint struct, the
+        operator's workspace).  item_size: at most that many locations per work item of the gather-scatter (default
+        OP_ITEM_SIZE; see operator_items).  owned (bool or uint8 per unknown, levels concatenated): the rows a rank of
+        the global solve owns.  Only the locations that contribute to an owned row are kept, so rhs, diag and A x are
+        those of the whole system on the owned rows and incomplete elsewhere; None keeps every location."""
         svh = self.svh
         dev = svh.device
         _lib.require_cuda(pos_xyz, "pos_xyz")
@@ -356,29 +359,41 @@ class KernelField(BaseField):
         S = int(item_size or OP_ITEM_SIZE)
         if S < 1:
             raise ValueError("item_size must be at least 1")
+        own8 = None
+        if owned is not None:
+            if owned.shape != (n,):
+                raise ValueError(f"owned must hold one entry per unknown ({n}), got shape {tuple(owned.shape)}")
+            own8 = owned.to(dev, torch.uint8).contiguous()
+            keep.append(own8)
         nb_op = call("nksr_op_workspace_bytes", svh.view(), cs, S)
         op_ws = torch.empty(nb_op, dtype=torch.uint8, device=dev)
         rhs = torch.empty(n, dtype=torch.float32, device=dev)
         diag = torch.empty(n, dtype=torch.float32, device=dev)
-        call("nksr_op_setup", svh.view(), self.feat_view(), cs, base_pos, base_nrm, key_pos, key_nrm, S, rhs, diag,
-             op_ws, nb_op, st)
+        call("nksr_op_setup", svh.view(), self.feat_view(), cs, base_pos, base_nrm, key_pos, key_nrm, own8, S, rhs,
+             diag, op_ws, nb_op, st)
         tm.mark("operator_setup")
+        kept = cs.n_pos + cs.n_nrm                          # without a mask every location is kept
+        if own8 is not None:                                # (a read-back: the kept count lives on the device)
+            layout = (C.c_int64 * 5)()
+            call("nksr_op_workspace_layout", svh.view(), cs, nb_op, C.addressof(layout))
+            kept = int(op_ws[layout[4]:layout[4] + 4].view(torch.int32).item())
         return SimpleNamespace(cs=cs, base_pos=base_pos, base_nrm=base_nrm, rhs=rhs, diag=diag, ws=op_ws,
-                               ws_bytes=nb_op, n=n, keep=keep, item_size=S,
+                               ws_bytes=nb_op, n=n, keep=keep, item_size=S, owned=own8, locations_kept=kept,
                                bytes_per_apply=operator_bytes_per_apply(svh, pos_xyz.shape[0], K, lines, self.channels,
                                                                         S))
 
     def operator_items(self, op):
-        """The work of a matrix_free_system, from its workspace: (order, vox, items).  order (m,) int32 is the merged
-        location order (r >= 0: sorted position r, ~r: sorted normal location r), vox (depth, m) their containing
-        voxels, items (count, 4) int32 the work items: begin, end in order, flags (1: first, 2: last item of its
-        top-level voxel), 0.  Reads the item count back to the host."""
-        out = (C.c_int64 * 4)()
+        """The work of a matrix_free_system, from its workspace: (order, vox, items).  order (kept,) int32 is the
+        merged order of the kept locations (r >= 0: sorted position r, ~r: sorted normal location r; every location
+        without an owned mask), vox (depth, kept) their containing voxels, items (count, 4) int32 the work items:
+        begin, end in order, flags (1: first, 2: last item of its top-level voxel), 0.  Reads the item count back to
+        the host."""
+        out = (C.c_int64 * 5)()
         call("nksr_op_workspace_layout", self.svh.view(), op.cs, op.ws_bytes, C.addressof(out))
         m = op.cs.n_pos + op.cs.n_nrm
         i32 = lambda off, cnt: op.ws[off:off + 4 * cnt].view(torch.int32)
-        count = int(i32(out[2], 1).item())
-        return i32(out[0], m), i32(out[1], self.svh.depth * m).view(self.svh.depth, m), \
+        count, kept = int(i32(out[2], 1).item()), int(i32(out[4], 1).item())
+        return i32(out[0], kept), i32(out[1], self.svh.depth * m).view(self.svh.depth, m)[:, :kept], \
             i32(out[3], 4 * count).view(count, 4)
 
     def apply_operator(self, op, x: torch.Tensor) -> torch.Tensor:

@@ -1,10 +1,12 @@
 """Multi-GPU check of nksr_b200/dist_solve.py (run under torchrun, one rank per GPU):
 
-    python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 tools/check_global_solve.py
+    python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 tools/check_global_solve.py \
+        [--operator assembled|matrix_free]
 
 Every rank builds the same seeded elongated cloud; the ranks solve ONE global system sharded by
 slabs (halo exchange + all-reduced dot products), rank 0 additionally solves the same system alone,
 and the coefficients are compared unknown by unknown through their (level, Morton key)."""
+import argparse
 import os
 import sys
 
@@ -28,6 +30,10 @@ def capsule(n, length=12.0, radius=0.5, seed=0):
 
 
 def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--operator", choices=("assembled", "matrix_free"), default=None,
+                    help="the global solve's operator (default: NKSR_OPERATOR, else assembled)")
+    args = ap.parse_args()
     rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
@@ -37,7 +43,7 @@ def main():
     W = 0.05
     rec = nksr_b200.Reconstructor(dev, tree_depth=3)
     t = lambda a: torch.from_numpy(a).to(dev)
-    field = ds.reconstruct_global(rec, t(xyz), t(nrm), W, halo_voxels=8, solver_tol=1e-6)
+    field = ds.reconstruct_global(rec, t(xyz), t(nrm), W, halo_voxels=8, solver_tol=1e-6, operator=args.operator)
     info = field.solve_info
     mesh = ds.extract_global_mesh(field, mise_iter=1)
     # owned coefficients with their (level, key) identity
@@ -50,7 +56,8 @@ def main():
     dist.all_gather_object(gathered, (mine, info))
     ok = True
     if rank == 0:
-        ref = ds.reconstruct_global(rec, t(xyz), t(nrm), W, halo_voxels=8, solver_tol=1e-6, group=solo)
+        ref = ds.reconstruct_global(rec, t(xyz), t(nrm), W, halo_voxels=8, solver_tol=1e-6, group=solo,
+                                    operator=args.operator)
         rk = torch.cat(ref.svh.keys).cpu().numpy()
         rl = np.concatenate([np.full(ref.svh.num_voxels(l), l) for l in range(3)])
         ra = ref.alpha.cpu().numpy()
@@ -61,7 +68,8 @@ def main():
             d = np.array([abs(lut[(int(l), int(k))] - float(a)) for l, k, a in zip(l_, k_, a_)])
             worst = max(worst, float(d.max()))
             print(f"rank {r}: owned {len(a_)} of local {inf['n']} unknowns, halo {inf['halo_recv']}, iters {inf['iterations']}, "
-                  f"relres {inf['relative_residual']:.2e}, slab {inf['slab']}, max |alpha - ref| = {d.max():.3e}")
+                  f"relres {inf['relative_residual']:.2e}, operator {inf['operator']}, kept locations "
+                  f"{inf.get('locations_kept')} of {inf.get('locations_total')}, slab {inf['slab']}, max |alpha - ref| = {d.max():.3e}")
         ok &= total == len(ra)                      # every unknown owned exactly once
         ok &= worst <= 2e-3 * scale
         refmesh = ref.extract_dual_mesh(mise_iter=1)
