@@ -7,14 +7,17 @@
 // where no voxel of a level <= kCutLevel continues (a single such voxel longer than S is an item of its own).
 //
 // k_op_walk: a persistent grid of warps steps over the items, lane = stencil slot.  Per location r the warp loads r's
-// lines of every level once, forms t_r = w_r E_r x (three values for a gradient location, one per axis) from the x
-// values of the containing voxel's 27 neighbours -- fetched once per run of locations with the same containing voxel
-// u_l, the next locations' nbr27 rows and x values requested under the current one's reductions -- and adds
-// E_l[r][s] t_r into a register accumulator per level.  When u_l changes, the accumulator is stored once to the planar
-// partial sums P[s][u] (27 planes of n floats).  A voxel of a level <= kCutLevel lies inside one item; a coarser voxel's
-// run may span items, and then every item stores its piece to an edge buffer, which k_op_edges sums in item order and
-// stores to P once.  No atomics: each P[.][u] has one writer, and the result is bitwise repeatable and independent of
-// the grid.  Voxels without locations are never written, and stay zero from the setup's clear.
+// lines of every level once (two locations ahead), forms t_r = w_r E_r x (three values for a gradient location, one
+// per axis) from the x values of the containing voxel's 27 neighbours -- fetched once per run of locations with the
+// same containing voxel u_l, one run ahead, their nbr27 rows two runs ahead -- and adds E_l[r][s] t_r into a register
+// accumulator per level.  The run bookkeeping is done per window of 32 locations, lane-parallel: one ballot per level
+// marks the run starts, and inside the window every branch is warp-uniform.  When u_l changes, the accumulator is
+// stored once to the planar partial sums P[s][u] (27 planes of n floats).  A voxel of a level <= kCutLevel lies inside
+// one item; a coarser voxel's run may span items, and then every item stores its piece to an edge buffer, which
+// k_op_edges sums in item order and stores to P once (whether a piece goes there is decided once per item).  The
+// stores to P go through a per-warp buffer in shared memory, 32 voxels at a time, one plane after the other.  No
+// atomics: each P[.][u] has one writer, and the result is bitwise repeatable and independent of the grid.  Voxels
+// without locations are never written, and stay zero from the setup's clear.
 //
 // k_op_apply: one thread per unknown, levels concatenated, grid-stride.  y_i = sum_s P[s][nbr27(i)[26 - s]] (u's slot s
 // is i exactly when i's slot 26 - s is u) + w_reg sum_s B3(d_s) <z_i, z_n> x_n over the 27 neighbours n = nbr27(i)[s]:
@@ -32,17 +35,12 @@ namespace {
 constexpr int kOpWarps = 4;          // warps per block of the walk
 constexpr int kApplyBlock = 256;
 constexpr int kEdgeBlock = 256;
-// items are cut at boundaries of the voxels of levels <= kCutLevel; the nbr27 rows / x values of levels below
-// kPrefetchLevels are requested two / one locations ahead (0: on demand, as each new containing voxel starts).  The
-// macros exist to measure the alternatives (DESIGN 4.2.1); the defaults are what the measurements chose.
+// items are cut at boundaries of the voxels of levels <= kCutLevel.  The macro exists to measure the alternatives
+// (DESIGN 4.2.1); the default is what the measurements chose.
 #ifndef NKSR_OP_CUT_LEVEL
 #define NKSR_OP_CUT_LEVEL 2
 #endif
-#ifndef NKSR_OP_PREFETCH_LEVELS
-#define NKSR_OP_PREFETCH_LEVELS 2
-#endif
 constexpr int kCutLevel = NKSR_OP_CUT_LEVEL;
-constexpr int kPrefetchLevels = NKSR_OP_PREFETCH_LEVELS;
 constexpr int kItemFirst = 1, kItemLast = 2;   // item flags: first / last item of its top voxel
 
 // row forms: value rows (positions), compact gradient lines (approx_kernel_grad), three full gradient rows
@@ -168,11 +166,45 @@ __global__ void k_op_cut(const int32_t* __restrict__ vox, int64_t m, const int2*
 }
 
 // ------------------------------------------------------------------------------------------- the walk of one item
+// The warp steps over the item in windows of 32 merged locations.  Each window is read lane-parallel (lane j =
+// location k0 + j: sequence entry and containing voxel per level), and one ballot per level marks where a run of
+// locations with the same containing voxel starts.  Inside the window every branch is warp-uniform: a run start is a
+// bit test, its voxel one shuffle.  The next window is held as well, so that a run start can find the next two runs
+// of its level in the run-start masks and request their x values and nbr27 rows one and two runs ahead.
+// A warp's finished partial sums on their way to P: up to 32 voxels, one row of 27 slots each (stride 33, so that both
+// the row-wise writes and the column-wise reads are free of bank conflicts), and the voxels' unknown indices.  A full
+// buffer is drained plane by plane: the buffered voxels are nearly consecutive, so each plane's store touches a few
+// sectors, where a voxel's own store would touch 27
+constexpr int kStage = 33;
+struct PStage {
+  float* v;     // [32][kStage] acc
+  float* d;     // [32][kStage] accd (setup)
+  int64_t* g;   // [32] offset[l] + u
+  int n;        // voxels held, warp-uniform
+};
+
+template <bool SETUP>
+__device__ __forceinline__ void op_stage_drain(const MfOperator& op, PStage& ps, int lane) {
+  __syncwarp();
+  if (lane < ps.n) {
+    const int64_t g = ps.g[lane];
+    float* p = op.P + g;
+    float* pd = SETUP ? op.Pd + g : nullptr;
+#pragma unroll 9
+    for (int s = 0; s < 27; ++s) {
+      p[(int64_t)s * op.n] = ps.v[lane * kStage + s];
+      if (SETUP) pd[(int64_t)s * op.n] = ps.d[lane * kStage + s];
+    }
+  }
+  __syncwarp();
+  ps.n = 0;
+}
+
 template <int NKIND, int MAXL, bool SETUP>
 __device__ __forceinline__ void op_walk_item(const MfOperator& op, const float* __restrict__ x, int it, int4 item,
-                                             EdgeBuffers eb, int lane) {
+                                             EdgeBuffers eb, PStage& ps, int lane) {
+  constexpr unsigned kAll = 0xffffffffu;
   constexpr int LINES = NKIND == kFull ? 3 : 1;     // 128-byte lines per (location, level) of the widest row
-  constexpr int PF = MAXL < kPrefetchLevels ? MAXL : kPrefetchLevels;
   const nksr_svh_t& svh = op.svh;
   const int L = svh.depth;
   const int cut = op_cut_level(L);
@@ -183,13 +215,22 @@ __device__ __forceinline__ void op_walk_item(const MfOperator& op, const float* 
   const CompactSpline spline(c_d27[sl][0], c_d27[sl][1], c_d27[sl][2]);
   const float inv_w0 = 1.f / svh.voxel_size;
 
-  // the voxels just before (lane l) and after (lane 16 + l) the item on level l, inside its top voxel
-  int edge_nb = -1;
-  if (lane < L && !(item.z & kItemFirst)) edge_nb = __ldg(vox + lane * m + b - 1);
-  else if (lane >= 16 && lane - 16 < L && !(item.z & kItemLast)) edge_nb = __ldg(vox + (lane - 16) * m + e);
+  // bit l (16 + l): the item's first (last) run on level l > cut continues from the previous (into the next) item
+  bool cont = false;
+  if (lane < L && !(item.z & kItemFirst)) {
+    const int p = __ldg(vox + lane * m + b - 1);
+    cont = p >= 0 && p == __ldg(vox + lane * m + b);
+  } else if (lane >= 16 && lane - 16 < L && !(item.z & kItemLast)) {
+    const int p = __ldg(vox + (lane - 16) * m + e);
+    cont = p >= 0 && p == __ldg(vox + (lane - 16) * m + e - 1);
+  }
+  const unsigned above = (0xffffu << (cut + 1)) & 0xffffu;
+  const unsigned edge = __ballot_sync(kAll, cont) & (above | above << 16);
 
-  // two windows of 32 merged locations: sequence entry and containing voxels, lane j = location k0 + j (+ 32)
-  int wq, wq2, wv[MAXL], wv2[MAXL];
+  // windows A (locations k0 + j) and B (k0 + 32 + j): sequence entry q, containing voxels v, and per level the run
+  // starts s (bit j: location j's voxel differs from the one before it; -1 before the item)
+  int qa, qb, va[MAXL], vb[MAXL];
+  unsigned sa[MAXL], sb[MAXL];
   auto load_win = [&](int k0, int& q, int (&v)[MAXL]) {
     const int k = k0 + lane;
     const bool in = k < e;
@@ -197,178 +238,186 @@ __device__ __forceinline__ void op_walk_item(const MfOperator& op, const float* 
 #pragma unroll
     for (int l = 0; l < MAXL; ++l) v[l] = (in && l < L) ? __ldg(vox + l * m + k) : -1;
   };
-  auto win = [&](int d, int v, int v2) {   // d = k - k0 in [0, 64), warp-uniform
-    return d < 32 ? __shfl_sync(0xffffffffu, v, d) : __shfl_sync(0xffffffffu, v2, d - 32);
+  auto starts_b = [&]() {   // B's run starts; B's lane 0 follows A's lane 31
+#pragma unroll
+    for (int l = 0; l < MAXL; ++l)
+      sb[l] = __ballot_sync(kAll, vb[l] != __shfl_sync(kAll, lane == 31 ? va[l] : vb[l], (lane + 31) & 31));
   };
-  int k0 = b;
-  load_win(b, wq, wv);
-  load_win(b + 32, wq2, wv2);
+  load_win(b, qa, va);
+  load_win(b + 32, qb, vb);
+#pragma unroll
+  for (int l = 0; l < MAXL; ++l) {
+    const int p = __shfl_up_sync(kAll, va[l], 1);
+    sa[l] = __ballot_sync(kAll, va[l] != (lane == 0 ? -1 : p));
+  }
+  starts_b();
 
-  float nx[MAXL][LINES];   // the next location's lines, requested one location ahead
-  auto load_lines = [&](int q, float (&dst)[MAXL][LINES]) {
+  // the lines of the next locations, requested AHEAD locations before they are visited: sequence entry, the lines
+  // of every level and (setup) the target values.  The three-line rows take one location, to stay in the registers
+  constexpr int AHEAD = NKIND == kFull ? 1 : 2;
+  constexpr int TN = SETUP ? 3 : 1;
+  struct Stage {
+    int q;
+    float ln[MAXL][LINES];
+    float tn[TN];
+  };
+  auto load_stage = [&](int q, Stage& s) {
+    s.q = q;
     if (q >= 0) {
       const float* p = op.cs.e_pos + (int64_t)q * L * NKSR_ROW_STRIDE + lane;
 #pragma unroll
       for (int l = 0; l < MAXL; ++l)
 #pragma unroll
-        for (int a = 0; a < LINES; ++a) dst[l][a] = (a == 0 && l < L) ? __ldcs(p + l * NKSR_ROW_STRIDE) : 0.f;
+        for (int a = 0; a < LINES; ++a) s.ln[l][a] = (a == 0 && l < L) ? __ldcs(p + l * NKSR_ROW_STRIDE) : 0.f;
+#pragma unroll
+      for (int a = 0; a < TN; ++a) s.tn[a] = 0.f;
     } else {
       const float* p = op.cs.e_nrm + (int64_t)~q * L * LINES * NKSR_ROW_STRIDE + lane;
 #pragma unroll
       for (int l = 0; l < MAXL; ++l)
 #pragma unroll
-        for (int a = 0; a < LINES; ++a) dst[l][a] = l < L ? __ldcs(p + (l * LINES + a) * NKSR_ROW_STRIDE) : 0.f;
+        for (int a = 0; a < LINES; ++a) s.ln[l][a] = l < L ? __ldcs(p + (l * LINES + a) * NKSR_ROW_STRIDE) : 0.f;
+#pragma unroll
+      for (int a = 0; a < TN; ++a) s.tn[a] = SETUP ? __ldg(op.cs.t_nrm + (int64_t)~q * 3 + a) : 0.f;
     }
   };
-
-  int cur[MAXL];
-  float acc[MAXL], accd[MAXL], xc[MAXL];
+  Stage st[AHEAD];
 #pragma unroll
-  for (int l = 0; l < MAXL; ++l) { cur[l] = -1; acc[l] = 0.f; accd[l] = 0.f; xc[l] = 0.f; }
-  unsigned first = 0xffffffffu;   // bit l: the current level-l run started at the item's first location
+  for (int s = 0; s < AHEAD; ++s) {
+    const int q = __shfl_sync(kAll, qa, s);
+    if (b + s < e) load_stage(q, st[s]);
+  }
 
-  // P[s][u] = acc, or the item's edge slot when u's run continues into the previous or the next item
+  // per level: the current run's voxel, accumulators and x values, the x values of the next run (xn) and the nbr27
+  // entry of the run after it (nn).  Bit l / 16 + l of req: they were requested (the run's start lay in the windows)
+  int cur[MAXL], nn[MAXL];
+  float acc[MAXL], accd[MAXL], xc[MAXL], xn[MAXL];
+#pragma unroll
+  for (int l = 0; l < MAXL; ++l) {
+    cur[l] = -1; nn[l] = -1;
+    acc[l] = 0.f; accd[l] = 0.f; xc[l] = 0.f; xn[l] = 0.f;
+  }
+  unsigned req = 0;
+  unsigned first = 0xffffffffu;   // bit l: the current level-l run started at the item's first location
+  auto nbr_of = [&](int l, int v) { return (v >= 0 && lane < 27) ? __ldg(svh.nbr27[l] + (int64_t)v * 27 + lane) : -1; };
+  auto x_of = [&](int l, int nb) { return nb >= 0 ? __ldg(x + svh.offset[l] + nb) : 0.f; };
+
+  // P[s][u] = acc through the warp's staging buffer, or the item's edge slot when u's run continues into the
+  // previous or the next item
   auto flush = [&](int l, bool last) {
-    const int u = cur[l];
-    bool to_edge = false;
-    int side = 0;
-    if (l > cut) {
-      const int pv = __shfl_sync(0xffffffffu, edge_nb, l), nv = __shfl_sync(0xffffffffu, edge_nb, 16 + l);
-      const bool f = (first >> l) & 1u;
-      to_edge = (f && pv == u) || (last && nv == u);
-      side = f ? 0 : 1;
-    }
-    if (lane < 27) {
-      if (to_edge) {
-        const int64_t q = (((int64_t)it * op.edge_levels + (l - cut - 1)) * 2 + side) * 27 + lane;
+    const bool f = (first >> l) & 1u;
+    const bool to_edge = (f && ((edge >> l) & 1u)) || (last && ((edge >> (16 + l)) & 1u));
+    if (to_edge) {
+      if (lane < 27) {
+        const int64_t q = (((int64_t)it * op.edge_levels + (l - cut - 1)) * 2 + (f ? 0 : 1)) * 27 + lane;
         eb.e[q] = acc[l];
         if (SETUP) eb.d[q] = accd[l];
-      } else {
-        const int64_t q = (int64_t)lane * op.n + svh.offset[l] + u;
-        op.P[q] = acc[l];
-        if (SETUP) op.Pd[q] = accd[l];
       }
+    } else {
+      if (lane < 27) {
+        ps.v[ps.n * kStage + lane] = acc[l];
+        if (SETUP) ps.d[ps.n * kStage + lane] = accd[l];
+      }
+      if (lane == 0) ps.g[ps.n] = svh.offset[l] + cur[l];
+      if (++ps.n == 32) op_stage_drain<SETUP>(op, ps, lane);
     }
   };
 
-  // pipelined levels: vk = v_l(k), vk1 = v_l(k + 1); xq = x at vk's stencil (requested when vk starts a run),
-  // nq = vk1's nbr27 entry (requested when vk1 starts a run)
-  constexpr int PFA = PF > 0 ? PF : 1;
-  int vk[PFA], vk1[PFA], nq[PFA];
-  float xq[PFA];
-#pragma unroll
-  for (int l = 0; l < PF; ++l) {
-    vk[l] = l < L ? win(0, wv[l], wv2[l]) : -1;
-    vk1[l] = (l < L && b + 1 < e) ? win(1, wv[l], wv2[l]) : -1;
-    xq[l] = 0.f;
-    nq[l] = -1;
-    if (!SETUP) {
-      const int nb = (vk[l] >= 0 && lane < 27) ? __ldg(svh.nbr27[l] + (int64_t)vk[l] * 27 + lane) : -1;
-      xq[l] = nb >= 0 ? __ldg(x + svh.offset[l] + nb) : 0.f;
-      nq[l] = (vk1[l] != vk[l] && vk1[l] >= 0 && lane < 27) ? __ldg(svh.nbr27[l] + (int64_t)vk1[l] * 27 + lane) : -1;
-    }
-  }
-  int q = win(0, wq, wq2);
-  load_lines(q, nx);
+  for (int k0 = b; k0 < e; k0 += 32) {
+    const int nj = e - k0 < 32 ? e - k0 : 32;
+    for (int j = 0; j < nj; ++j) {
+      const int k = k0 + j;
+      Stage nx;
+      {
+        const int ja = j + AHEAD;
+        const int q = __shfl_sync(kAll, ja < 32 ? qa : qb, ja & 31);
+        if (k + AHEAD < e) load_stage(q, nx);
+      }
 
-  for (int k = b; k < e; ++k) {
-    float ln[MAXL][LINES];
+      // runs starting at this location: the finished run goes out, the new one's x values come in, and the next
+      // two runs' x values and nbr27 rows are requested
 #pragma unroll
-    for (int l = 0; l < MAXL; ++l)
-#pragma unroll
-      for (int a = 0; a < LINES; ++a) ln[l][a] = nx[l][a];
-    const int qn = k + 1 < e ? win(k + 1 - k0, wq, wq2) : 0;
-    if (k + 1 < e) load_lines(qn, nx);
-
-    // a new containing voxel: the finished run goes out, the new one's x values come in
-#pragma unroll
-    for (int l = 0; l < MAXL; ++l) {
-      if (l < L) {
-        const int v = l < PF ? vk[l < PF ? l : 0] : win(k - k0, wv[l], wv2[l]);
-        if (v != cur[l]) {
+      for (int l = 0; l < MAXL; ++l) {
+        if (l < L && ((sa[l] >> j) & 1u)) {
+          const int v = __shfl_sync(kAll, va[l], j);
           if (cur[l] >= 0) flush(l, false);
           if (k > b) first &= ~(1u << l);
           cur[l] = v;
           acc[l] = 0.f;
           accd[l] = 0.f;
           if (!SETUP) {
-            if (l < PF) {
-              xc[l] = xq[l < PF ? l : 0];
-            } else {
-              const int nb = (v >= 0 && lane < 27) ? __ldg(svh.nbr27[l] + (int64_t)v * 27 + lane) : -1;
-              xc[l] = nb >= 0 ? __ldg(x + svh.offset[l] + nb) : 0.f;
-            }
+            xc[l] = v < 0 ? 0.f : ((req >> l) & 1u) ? xn[l] : x_of(l, nbr_of(l, v));
+            uint64_t rest = ((uint64_t)sb[l] << 32 | sa[l]) & (~0ull << (j + 1));
+            const int j1 = __ffsll((long long)rest) - 1;
+            rest &= rest - 1;
+            const int j2 = __ffsll((long long)rest) - 1;
+            const int v1 = __shfl_sync(kAll, j1 < 32 ? va[l] : vb[l], j1 & 31);
+            const int v2 = __shfl_sync(kAll, j2 < 32 ? va[l] : vb[l], j2 & 31);
+            // the next run is the one whose nbr27 entry the previous run start requested, when it found it
+            xn[l] = j1 < 0 ? 0.f : x_of(l, ((req >> (16 + l)) & 1u) ? nn[l] : nbr_of(l, v1));
+            nn[l] = j2 < 0 ? -1 : nbr_of(l, v2);
+            req = (req & ~(0x10001u << l)) | (j1 >= 0 ? 1u << l : 0u) | (j2 >= 0 ? 0x10000u << l : 0u);
           }
         }
       }
-    }
-    // requested under this location's reductions: x for location k + 1, nbr27 for location k + 2
-#pragma unroll
-    for (int l = 0; l < PF; ++l) {
-      if (l < L) {
-        const int v2 = k + 2 < e ? win(k + 2 - k0, wv[l], wv2[l]) : -1;
-        if (!SETUP) {
-          xq[l] = (vk1[l] != vk[l] && nq[l] >= 0) ? __ldg(x + svh.offset[l] + nq[l]) : 0.f;
-          nq[l] = (v2 != vk1[l] && v2 >= 0 && lane < 27) ? __ldg(svh.nbr27[l] + (int64_t)v2 * 27 + lane) : -1;
-        }
-        vk[l] = vk1[l];
-        vk1[l] = v2;
-      }
-    }
 
-    // this location's rows: t = w E x, then acc += E t
-    auto visit = [&](auto kind_tag) {
-      constexpr int KIND = decltype(kind_tag)::value;
-      constexpr int AX = KIND == kValue ? 1 : 3;
-      const float w = KIND == kValue ? op.cs.w_pos : op.cs.w_nrm;
-      float ev[MAXL][AX];   // zero on a level without containing voxel, and in lanes >= 27
+      // this location's rows: t = w E x, then acc += E t
+      const Stage& cs = st[0];
+      auto visit = [&](auto kind_tag) {
+        constexpr int KIND = decltype(kind_tag)::value;
+        constexpr int AX = KIND == kValue ? 1 : 3;
+        const float w = KIND == kValue ? op.cs.w_pos : op.cs.w_nrm;
+        float ev[MAXL][AX];   // zero on a level without containing voxel, and in lanes >= 27
 #pragma unroll
-      for (int l = 0; l < MAXL; ++l) {
-        if (KIND == kCompact) {
-          float e0 = 0.f, e1 = 0.f, e2 = 0.f;
-          if (l < L) spline.grad_rows(ln[l][0], inv_w0 * __int_as_float((127 - l) << 23), lane, e0, e1, e2);
-          ev[l][0] = e0;
-          ev[l][AX > 1 ? 1 : 0] = e1;
-          ev[l][AX > 2 ? 2 : 0] = e2;
+        for (int l = 0; l < MAXL; ++l) {
+          if (KIND == kCompact) {
+            float e0 = 0.f, e1 = 0.f, e2 = 0.f;
+            if (l < L) spline.grad_rows(cs.ln[l][0], inv_w0 * __int_as_float((127 - l) << 23), lane, e0, e1, e2);
+            ev[l][0] = e0;
+            ev[l][AX > 1 ? 1 : 0] = e1;
+            ev[l][AX > 2 ? 2 : 0] = e2;
+          } else {
+#pragma unroll
+            for (int a = 0; a < AX; ++a) ev[l][a] = cs.ln[l][a];
+          }
+        }
+        float t[AX];
+        if (SETUP) {
+#pragma unroll
+          for (int a = 0; a < AX; ++a) t[a] = KIND == kValue ? 0.f : w * cs.tn[a < TN ? a : 0];
         } else {
 #pragma unroll
-          for (int a = 0; a < AX; ++a) ev[l][a] = ln[l][a];
-        }
-      }
-      float t[AX];
-      if (SETUP) {
+          for (int a = 0; a < AX; ++a) {
+            float s = 0.f;
 #pragma unroll
-        for (int a = 0; a < AX; ++a) t[a] = KIND == kValue ? 0.f : w * __ldg(op.cs.t_nrm + (int64_t)~q * 3 + a);
-      } else {
+            for (int l = 0; l < MAXL; ++l) s = fmaf(ev[l][a], xc[l], s);
+            t[a] = s;
+          }
 #pragma unroll
-        for (int a = 0; a < AX; ++a) {
-          float s = 0.f;
-#pragma unroll
-          for (int l = 0; l < MAXL; ++l) s = fmaf(ev[l][a], xc[l], s);
-          t[a] = s;
+          for (int a = 0; a < AX; ++a) t[a] = w * warp_sum(t[a]);
         }
 #pragma unroll
-        for (int a = 0; a < AX; ++a) t[a] = w * warp_sum(t[a]);
-      }
+        for (int l = 0; l < MAXL; ++l) {
 #pragma unroll
-      for (int l = 0; l < MAXL; ++l) {
-#pragma unroll
-        for (int a = 0; a < AX; ++a) {
-          acc[l] = fmaf(ev[l][a], t[a], acc[l]);
-          if (SETUP) accd[l] = fmaf(w * ev[l][a], ev[l][a], accd[l]);
+          for (int a = 0; a < AX; ++a) {
+            acc[l] = fmaf(ev[l][a], t[a], acc[l]);
+            if (SETUP) accd[l] = fmaf(w * ev[l][a], ev[l][a], accd[l]);
+          }
         }
-      }
-    };
-    if (q >= 0) visit(std::integral_constant<int, kValue>());
-    else visit(std::integral_constant<int, NKIND>());
+      };
+      if (cs.q >= 0) visit(std::integral_constant<int, kValue>());
+      else visit(std::integral_constant<int, NKIND>());
 
-    q = qn;
-    if (k + 1 - k0 == 32) {   // slide the windows
-      k0 += 32;
-      wq = wq2;
 #pragma unroll
-      for (int l = 0; l < MAXL; ++l) wv[l] = wv2[l];
-      load_win(k0 + 32, wq2, wv2);
+      for (int s = 0; s + 1 < AHEAD; ++s) st[s] = st[s + 1];
+      st[AHEAD - 1] = nx;
+    }
+    if (k0 + 32 < e) {   // slide the windows
+      qa = qb;
+#pragma unroll
+      for (int l = 0; l < MAXL; ++l) { va[l] = vb[l]; sa[l] = sb[l]; }
+      load_win(k0 + 64, qb, vb);
+      starts_b();
     }
   }
 #pragma unroll
@@ -377,14 +426,28 @@ __device__ __forceinline__ void op_walk_item(const MfOperator& op, const float* 
 }
 
 template <int NKIND, int MAXL, bool SETUP>
-__global__ void __launch_bounds__(kOpWarps * 32, MAXL <= 4 ? 5 : 1)   // depth <= 4: at most 102 registers
+// depth <= 4: at most 102 registers for the application (5 blocks per SM), 128 for the setup walk, which holds the
+// diagonal's accumulators and buffer as well (4 blocks per SM)
+__global__ void __launch_bounds__(kOpWarps * 32, MAXL <= 4 ? (SETUP ? 4 : 5) : 1)
 k_op_walk(MfOperator op, const float* __restrict__ x, const int* __restrict__ done) {
+  __shared__ float s_v[kOpWarps][SETUP ? 2 : 1][32 * kStage];
+  __shared__ int64_t s_g[kOpWarps][32];
   if (done && *done) return;
-  const int lane = threadIdx.x & 31;
-  const int n_items = *op.n_items;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  PStage ps{s_v[warp][0], SETUP ? s_v[warp][SETUP ? 1 : 0] : nullptr, s_g[warp], 0};
+  // the warp's item index and bounds through redux.sync: warp-uniform values, and the compiler sees them as such
+  const int n_items = (int)__reduce_max_sync(0xffffffffu, (unsigned)*op.n_items);
   const EdgeBuffers eb = op_edge_buffers(op);
-  for (int it = blockIdx.x * kOpWarps + (threadIdx.x >> 5); it < n_items; it += gridDim.x * kOpWarps)
-    op_walk_item<NKIND, MAXL, SETUP>(op, x, it, op.items[it], eb, lane);
+  for (int it = (int)__reduce_max_sync(0xffffffffu, blockIdx.x * kOpWarps + warp); it < n_items;
+       it += gridDim.x * kOpWarps) {
+    const int4 item = op.items[it];
+    op_walk_item<NKIND, MAXL, SETUP>(op, x, it,
+                                     make_int4((int)__reduce_max_sync(0xffffffffu, (unsigned)item.x),
+                                               (int)__reduce_max_sync(0xffffffffu, (unsigned)item.y),
+                                               (int)__reduce_max_sync(0xffffffffu, (unsigned)item.z), 0),
+                                     eb, ps, lane);
+  }
+  if (ps.n > 0) op_stage_drain<SETUP>(op, ps, lane);
 }
 
 // one warp per (item, level above the cut): a run that starts in the item and continues into the next ones is summed
@@ -597,10 +660,25 @@ int sm_count() {
   return sms > 0 ? sms : 132;
 }
 
+// resident blocks per SM of the walk kernel this operator launches
+template <bool SETUP>
+int walk_blocks_per_sm(const MfOperator& op) {
+  const bool compact = op.cs.nrm_compact == 1, deep = op.svh.depth > 4;
+  const void* f = deep ? (compact ? (const void*)k_op_walk<kCompact, NKSR_MAX_DEPTH, SETUP>
+                                  : (const void*)k_op_walk<kFull, NKSR_MAX_DEPTH, SETUP>)
+                       : (compact ? (const void*)k_op_walk<kCompact, 4, SETUP> : (const void*)k_op_walk<kFull, 4, SETUP>);
+  int blocks = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, f, kOpWarps * 32, 0) != cudaSuccess || blocks < 1)
+    blocks = 1;
+  return blocks;
+}
+
 template <bool SETUP>
 void walk_launch(const MfOperator& op, const float* x, const int* done, cudaStream_t s) {
   const bool compact = op.cs.nrm_compact == 1;
-#define NKSR_WALK(NK, ML) k_op_walk<NK, ML, SETUP><<<op.walk_grid, kOpWarps * 32, 0, s>>>(op, x, done)
+  // the setup walk, once per solve, has its own occupancy (see k_op_walk)
+  const int grid = SETUP ? sm_count() * walk_blocks_per_sm<true>(op) : op.walk_grid;
+#define NKSR_WALK(NK, ML) k_op_walk<NK, ML, SETUP><<<grid, kOpWarps * 32, 0, s>>>(op, x, done)
   if (op.svh.depth <= 4) {
     if (compact) NKSR_WALK(kCompact, 4); else NKSR_WALK(kFull, 4);
   } else {
@@ -608,18 +686,6 @@ void walk_launch(const MfOperator& op, const float* x, const int* done, cudaStre
   }
 #undef NKSR_WALK
   if (op.edge_levels > 0) k_op_edges<SETUP><<<op.edge_grid, kEdgeBlock, 0, s>>>(op, done);
-}
-
-// resident blocks per SM of the walk kernel this operator launches
-int walk_blocks_per_sm(const MfOperator& op) {
-  const bool compact = op.cs.nrm_compact == 1, deep = op.svh.depth > 4;
-  const void* f = deep ? (compact ? (const void*)k_op_walk<kCompact, NKSR_MAX_DEPTH, false>
-                                  : (const void*)k_op_walk<kFull, NKSR_MAX_DEPTH, false>)
-                       : (compact ? (const void*)k_op_walk<kCompact, 4, false> : (const void*)k_op_walk<kFull, 4, false>);
-  int blocks = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, f, kOpWarps * 32, 0) != cudaSuccess || blocks < 1)
-    blocks = 1;
-  return blocks;
 }
 
 bool op_valid(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c, const int32_t* base_pos,
@@ -661,7 +727,7 @@ MfOperator make_op(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_co
   op.max_items = reinterpret_cast<int64_t*>(w + o.max_items);
   op.items = reinterpret_cast<int4*>(w + o.fixed);
   const int sms = sm_count();
-  op.walk_grid = sms * walk_blocks_per_sm(op);
+  op.walk_grid = sms * walk_blocks_per_sm<false>(op);
   op.edge_grid = sms * 8;
   return op;
 }
