@@ -312,6 +312,15 @@ NKSR_API int nksr_op_setup(const nksr_svh_t* svh, const nksr_feat_t* feat, const
 NKSR_API int nksr_op_apply(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_constraints_t* c,
                            const int32_t* base_pos, const int32_t* base_nrm, const float* x, float* y, void* ws,
                            size_t ws_bytes, void* stream);
+/* The constraint values the backward of a matrix-free solve needs (DESIGN 4.6), read from the kernel rows of c (the
+ * rows nksr_op_setup used: e_pos, e_nrm with nrm_compact 0 or 1) at the same sorted locations, for two vectors x0, x1
+ * (n unknowns each, levels concatenated): out_pos[j][k] = E_j x_k for every sorted position j, out_nrm[j][k][a] = the
+ * gradient row a of sorted normal location j times x_k.  No weights are applied.  base_pos / base_nrm as for
+ * nksr_op_setup; a location without containing voxel on a level gets nothing from it.  One warp per location, no
+ * atomics: bitwise repeatable.  Needs no operator workspace. */
+NKSR_API int nksr_op_constraint_values(const nksr_svh_t* svh, const nksr_constraints_t* c, const int32_t* base_pos,
+                                       const int32_t* base_nrm, const float* x0, const float* x1, float* out_pos,
+                                       float* out_nrm, void* stream);
 /* out[5] (host) = byte offsets in a workspace of ws_bytes bytes of the merged location order ([m] int32: r >= 0 position
  * r, ~r normal location r; its first `kept` entries are used), its containing voxels ([depth][m] int32), the item
  * count (int32), the items ([count] int4: begin, end, flags 1 first / 2 last item of its top-level voxel, 0) and the

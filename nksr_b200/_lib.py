@@ -100,6 +100,7 @@ _SIGNATURES = {
     "nksr_op_setup": ("i", "SFK" + "pppppi" + "pppzp"),
     "nksr_op_apply": ("i", "SFK" + "pppppzp"),
     "nksr_op_workspace_layout": ("i", "SKzp"),
+    "nksr_op_constraint_values": ("i", "SKpppppp" + "p"),
     "nksr_pcg_solve_matrix_free": ("i", "SFK" + "ppppp" + "fiii" + "pzpzdp"),
     "nksr_dcg_workspace_bytes": ("z", ""),
     "nksr_dcg_init": ("i", "pppppppp" + "q" + "pz" + "pp"),

@@ -603,6 +603,95 @@ k_op_apply_dcg(nksr_svh_t svh, nksr_feat_t feat, float w_reg, const float* __res
   }
 }
 
+// ------------------------------------------------------------------------------- constraint values for the backward
+// E_j x0 and E_j x1 at location j (KIND kValue: one value row; kCompact / kFull: the three gradient rows), read from the
+// resident rows: one warp, lane = stencil slot.  Per level the containing voxel, then its nbr27 entry and the lines,
+// then the x values of both vectors are requested for every level before any is used; each line is read once and
+// serves both vectors.  A level without containing voxel contributes nothing.  The per-lane sums run over the levels in
+// ascending order and are then reduced over the warp, the order of the walk's t_r: E_j x here is bitwise the walk's.
+// out (2 x AX floats at j): the AX values of x0, then those of x1
+template <int KIND, int MAXL>
+__device__ __forceinline__ void op_location_values(const nksr_svh_t& svh, const float* __restrict__ rows,
+                                                   const int32_t* __restrict__ base, int64_t nb, int64_t j,
+                                                   const float* __restrict__ x0, const float* __restrict__ x1,
+                                                   float* __restrict__ out, int lane) {
+  constexpr int AX = KIND == kValue ? 1 : 3;
+  constexpr int LINES = KIND == kFull ? 3 : 1;
+  const int L = svh.depth;
+  int v[MAXL];
+#pragma unroll
+  for (int l = 0; l < MAXL; ++l) v[l] = l < L ? __ldg(base + l * nb + j) : -1;
+  const float* p = rows + j * L * LINES * NKSR_ROW_STRIDE + lane;
+  int nbr[MAXL];
+  float ln[MAXL][LINES];
+#pragma unroll
+  for (int l = 0; l < MAXL; ++l) {
+    nbr[l] = (v[l] >= 0 && lane < 27) ? __ldg(svh.nbr27[l] + (int64_t)v[l] * 27 + lane) : -1;
+#pragma unroll
+    for (int a = 0; a < LINES; ++a) ln[l][a] = v[l] >= 0 ? __ldcs(p + (l * LINES + a) * NKSR_ROW_STRIDE) : 0.f;
+  }
+  float xa[MAXL], xb[MAXL];
+#pragma unroll
+  for (int l = 0; l < MAXL; ++l) {
+    const int64_t g = nbr[l] >= 0 ? svh.offset[l] + nbr[l] : -1;
+    xa[l] = g >= 0 ? __ldg(x0 + g) : 0.f;
+    xb[l] = g >= 0 ? __ldg(x1 + g) : 0.f;
+  }
+  const int sl = lane < 27 ? lane : 13;
+  const CompactSpline spline(c_d27[sl][0], c_d27[sl][1], c_d27[sl][2]);
+  const float inv_w0 = 1.f / svh.voxel_size;
+  float sa[AX], sb[AX];
+#pragma unroll
+  for (int a = 0; a < AX; ++a) sa[a] = sb[a] = 0.f;
+#pragma unroll
+  for (int l = 0; l < MAXL; ++l) {
+    float ev[AX];
+    if (KIND == kCompact) {
+      float e0 = 0.f, e1 = 0.f, e2 = 0.f;
+      if (l < L) spline.grad_rows(ln[l][0], inv_w0 * __int_as_float((127 - l) << 23), lane, e0, e1, e2);
+      ev[0] = e0;
+      ev[AX > 1 ? 1 : 0] = e1;
+      ev[AX > 2 ? 2 : 0] = e2;
+    } else {
+#pragma unroll
+      for (int a = 0; a < AX; ++a) ev[a] = ln[l][a < LINES ? a : 0];
+    }
+#pragma unroll
+    for (int a = 0; a < AX; ++a) {
+      sa[a] = fmaf(ev[a], xa[l], sa[a]);
+      sb[a] = fmaf(ev[a], xb[l], sb[a]);
+    }
+  }
+#pragma unroll
+  for (int a = 0; a < AX; ++a) {
+    sa[a] = warp_sum(sa[a]);
+    sb[a] = warp_sum(sb[a]);
+  }
+  if (lane == 0) {
+#pragma unroll
+    for (int a = 0; a < AX; ++a) {
+      out[a] = sa[a];
+      out[AX + a] = sb[a];
+    }
+  }
+}
+
+// one warp per location: the sorted positions, then the sorted normal locations
+template <int NKIND, int MAXL>
+__global__ void __launch_bounds__(kApplyBlock)
+k_op_constraint_values(nksr_svh_t svh, nksr_constraints_t cs, const int32_t* __restrict__ base_pos,
+                       const int32_t* __restrict__ base_nrm, const float* __restrict__ x0,
+                       const float* __restrict__ x1, float* __restrict__ out_pos, float* __restrict__ out_nrm) {
+  const int lane = threadIdx.x & 31;
+  const int64_t i = (blockIdx.x * (int64_t)kApplyBlock + threadIdx.x) >> 5;
+  if (i < cs.n_pos) {
+    op_location_values<kValue, MAXL>(svh, cs.e_pos, base_pos, cs.n_pos, i, x0, x1, out_pos + 2 * i, lane);
+  } else if (i < cs.n_pos + cs.n_nrm) {
+    const int64_t j = i - cs.n_pos;
+    op_location_values<NKIND, MAXL>(svh, cs.e_nrm, base_nrm, cs.n_nrm, j, x0, x1, out_nrm + 6 * j, lane);
+  }
+}
+
 // -------------------------------------------------------------------------------------------------------- host side
 size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
 
@@ -833,6 +922,32 @@ int nksr_op_apply(const nksr_svh_t* svh, const nksr_feat_t* feat, const nksr_con
   const int rc = mf_operator_make(svh, feat, c, base_pos, base_nrm, ws, ws_bytes, &op);
   if (rc != NKSR_OK) return rc;
   mf_apply_launch(op, x, y, nullptr, grid_for(op.n, kApplyBlock), nullptr, as_stream(stream));
+  NKSR_CHECK_LAUNCH();
+  return NKSR_OK;
+}
+
+int nksr_op_constraint_values(const nksr_svh_t* svh, const nksr_constraints_t* c, const int32_t* base_pos,
+                              const int32_t* base_nrm, const float* x0, const float* x1, float* out_pos,
+                              float* out_nrm, void* stream) {
+  if (!svh || !c || svh->depth < 1 || svh->depth > NKSR_MAX_DEPTH || !x0 || !x1) return NKSR_E_INVALID;
+  if (c->nrm_compact != 0 && c->nrm_compact != 1) return NKSR_E_INVALID;
+  if (c->n_pos < 0 || c->n_nrm < 0) return NKSR_E_INVALID;
+  if (c->n_pos > 0 && (!c->e_pos || !base_pos || !out_pos)) return NKSR_E_INVALID;
+  if (c->n_nrm > 0 && (!c->e_nrm || !base_nrm || !out_nrm)) return NKSR_E_INVALID;
+  for (int l = 0; l < svh->depth; ++l)
+    if (svh->n[l] > 0 && !svh->nbr27[l]) return NKSR_E_INVALID;
+  const int64_t m = c->n_pos + c->n_nrm;
+  if (m == 0) return NKSR_OK;
+  const int grid = grid_for(m * 32, kApplyBlock);
+  cudaStream_t s = as_stream(stream);
+#define NKSR_VALUES(NK, ML) \
+  k_op_constraint_values<NK, ML><<<grid, kApplyBlock, 0, s>>>(*svh, *c, base_pos, base_nrm, x0, x1, out_pos, out_nrm)
+  if (svh->depth <= 4) {
+    if (c->nrm_compact == 1) NKSR_VALUES(kCompact, 4); else NKSR_VALUES(kFull, 4);
+  } else {
+    if (c->nrm_compact == 1) NKSR_VALUES(kCompact, NKSR_MAX_DEPTH); else NKSR_VALUES(kFull, NKSR_MAX_DEPTH);
+  }
+#undef NKSR_VALUES
   NKSR_CHECK_LAUNCH();
   return NKSR_OK;
 }

@@ -284,9 +284,10 @@ class KernelField(BaseField):
         or 'assembled' (the CSR Gram matrix).  Default: matrix-free with approx_kernel_grad (compact rows) on systems of
         at least MATRIX_FREE_MIN_UNKNOWNS unknowns, assembled otherwise.  A Gram fill chosen explicitly
         (solver_config['fill'] or NKSR_FILL) asks for the matrix that fill builds, so it too selects the assembled
-        operator unless the operator is given as well.  Grad-recording solves and keep_system always assemble.  The
-        global solve (dist_solve.reconstruct_global) takes the operator as an argument or from NKSR_OPERATOR, and
-        assembles when neither names one."""
+        operator unless the operator is given as well.  keep_system always assembles.  Grad-recording solves do not
+        use this rule: they take the operator from _grad_operator, which reads the explicit names only.  The global
+        solve (dist_solve.reconstruct_global) takes the operator as an argument or from NKSR_OPERATOR, and assembles
+        when neither names one."""
         op = self.solver_config.get("operator") or os.environ.get("NKSR_OPERATOR")
         if op is None:
             big = self.svh.num_unknowns >= MATRIX_FREE_MIN_UNKNOWNS
@@ -296,11 +297,25 @@ class KernelField(BaseField):
             raise ValueError("solver_config['operator'] must be 'matrix_free' or 'assembled'")
         return op
 
+    def _grad_operator(self):
+        """The operator of a grad-recording solve (_KernelSolve): 'matrix_free' only when solver_config['operator'] or
+        NKSR_OPERATOR names it, else 'assembled'.  The size rule of _operator was measured on inference solves and does
+        not apply here.  keep_system always assembles."""
+        op = self.solver_config.get("operator") or os.environ.get("NKSR_OPERATOR") or "assembled"
+        if op not in ("matrix_free", "assembled"):
+            raise ValueError("solver_config['operator'] must be 'matrix_free' or 'assembled'")
+        return "assembled" if self.solver_config.get("keep_system") else op
+
     def _solve_matrix_free(self, pos_xyz, normal_xyz, normal_value, pos_weight, normal_weight, reg_weight):
         """Jacobi-PCG on A = E^T W E + reg R without assembling A (DESIGN 4.2.1): kernel rows (compact gradient lines
         with approx_kernel_grad), then rhs and diagonal (nksr_op_setup), then the PCG, whose every iteration applies A
         from the rows (nksr_pcg_solve_matrix_free).  No count, placement, blocks or fill; solve_info['nnz'] = 0."""
         op = self.matrix_free_system(pos_xyz, normal_xyz, normal_value, pos_weight, normal_weight, reg_weight)
+        return self._pcg_matrix_free(op, op.rhs)
+
+    def _pcg_matrix_free(self, op, rhs, adjoint: bool = False):
+        """Jacobi-PCG on the operator of a matrix_free_system: the forward solve (A alpha = b) and the adjoint solve of
+        the backward (A lambda = dL/dalpha) run on the same workspace.  Reports as _pcg does."""
         svh, dev, n = self.svh, self.svh.device, op.n
         alpha = torch.empty(n, dtype=torch.float32, device=dev)
         info = (C.c_double * 8)()
@@ -308,21 +323,34 @@ class KernelField(BaseField):
         nb = call("nksr_pcg_workspace_bytes", n)
         ws = torch.empty(nb, dtype=torch.uint8, device=dev)
         call("nksr_pcg_solve_matrix_free", svh.view(), self.feat_view(), op.cs, op.base_pos, op.base_nrm, op.diag,
-             op.rhs, alpha, float(self.solver_config["tol"]), int(self.solver_config["max_iter"]),
+             rhs, alpha, float(self.solver_config["tol"]), int(self.solver_config["max_iter"]),
              int(self.solver_config["check_every"]), profile, op.ws, op.ws_bytes, ws, nb, info, stream_ptr(dev))
         tm = getattr(self, "_timer", None) or _lib.StageTimer(dev, enabled=False)
-        tm.mark("pcg")
-        self._pcg_report(info, n, 0, False, operator="matrix_free", operator_bytes_per_apply=op.bytes_per_apply)
+        tm.mark("adjoint_pcg" if adjoint else "pcg")
+        self._pcg_report(info, n, 0, adjoint, operator="matrix_free", operator_bytes_per_apply=op.bytes_per_apply)
         return alpha
 
+    def constraint_values(self, op, x0: torch.Tensor, x1: torch.Tensor):
+        """E_j x0 and E_j x1 at the sorted constraint locations of a matrix_free_system, read from its kernel rows
+        (nksr_op_constraint_values): (n_pos, 2) values of the sorted positions and (n_nrm, 2, 3) gradient rows of the
+        sorted normal locations, for x0 then x1.  No weights."""
+        dev = self.svh.device
+        vp = torch.empty((op.cs.n_pos, 2), dtype=torch.float32, device=dev)
+        vn = torch.empty((op.cs.n_nrm, 2, 3), dtype=torch.float32, device=dev)
+        call("nksr_op_constraint_values", self.svh.view(), op.cs, op.base_pos, op.base_nrm,
+             x0.to(torch.float32).contiguous(), x1.to(torch.float32).contiguous(), vp, vn, stream_ptr(dev))
+        return vp, vn
+
     def matrix_free_system(self, pos_xyz, normal_xyz=None, normal_value=None, pos_weight=1.0, normal_weight=1.0,
-                           reg_weight=1.0, item_size: Optional[int] = None, owned: Optional[torch.Tensor] = None):
+                           reg_weight=1.0, item_size: Optional[int] = None, owned: Optional[torch.Tensor] = None,
+                           keep_constraints: bool = False):
         """Kernel rows of the sorted constraint locations and the operator's setup (nksr_op_setup): returns
         .rhs, .diag, .n, .locations_kept and what apply_operator needs (the rows, the constraint struct, the
         operator's workspace).  item_size: at most that many locations per work item of the gather-scatter (default
         OP_ITEM_SIZE; see operator_items).  owned (bool or uint8 per unknown, levels concatenated): the rows a rank of
         the global solve owns.  Only the locations that contribute to an owned row are kept, so rhs, diag and A x are
-        those of the whole system on the owned rows and incomplete elsewhere; None keeps every location."""
+        those of the whole system on the owned rows and incomplete elsewhere; None keeps every location.
+        keep_constraints: also `.cons`, the record assemble(keep_constraints=True) returns (what the backward needs)."""
         svh = self.svh
         dev = svh.device
         _lib.require_cuda(pos_xyz, "pos_xyz")
@@ -338,6 +366,9 @@ class KernelField(BaseField):
         _, _, base_pos, range_pos, e_pos = self._sorted_rows(pos_xyz, 0, loc=loc_pos)
         cs.e_pos, cs.range_pos, cs.n_pos, cs.w_pos = e_pos.data_ptr(), range_pos.data_ptr(), pos_xyz.shape[0], float(pos_weight)
         keep = [e_pos, range_pos, key_pos]
+        cons = SimpleNamespace(pos=(loc_pos[1], loc_pos[3], loc_pos[4]),
+                               nrm=None, perm_nrm=None, w_pos=float(pos_weight), w_nrm=float(normal_weight),
+                               w_reg=float(reg_weight)) if keep_constraints else None
         base_nrm, key_nrm, lines, K = None, None, 0, 0
         if normal_xyz is not None and normal_xyz.shape[0] > 0:
             normal_xyz = normal_xyz.detach().to(dev, torch.float32).contiguous()
@@ -345,6 +376,8 @@ class KernelField(BaseField):
             mode = 2 if self.approx_kernel_grad else 1          # compact lines: one 128 B line per location and level
             *loc_nrm, key_nrm = self._sorted_locations(normal_xyz, normal_value, with_keys=True)
             _, t_nrm, base_nrm, range_nrm, e_nrm = self._sorted_rows(normal_xyz, mode, normal_value, loc=loc_nrm)
+            if cons is not None:
+                cons.nrm, cons.t_nrm, cons.perm_nrm = (loc_nrm[1], loc_nrm[3], loc_nrm[4]), t_nrm, loc_nrm[0]
             keep += [t_nrm, range_nrm, e_nrm, key_nrm]
             cs.e_nrm, cs.range_nrm, cs.t_nrm = e_nrm.data_ptr(), range_nrm.data_ptr(), t_nrm.data_ptr()
             K, lines = normal_xyz.shape[0], (1 if mode == 2 else 3)
@@ -380,7 +413,7 @@ class KernelField(BaseField):
         return SimpleNamespace(cs=cs, base_pos=base_pos, base_nrm=base_nrm, rhs=rhs, diag=diag, ws=op_ws,
                                ws_bytes=nb_op, n=n, keep=keep, item_size=S, owned=own8, locations_kept=kept,
                                bytes_per_apply=operator_bytes_per_apply(svh, pos_xyz.shape[0], K, lines, self.channels,
-                                                                        S))
+                                                                        S), cons=cons)
 
     def operator_items(self, op):
         """The work of a matrix_free_system, from its workspace: (order, vox, items).  order (kept,) int32 is the
@@ -712,12 +745,23 @@ class _KernelSolve(torch.autograd.Function):
     Backward, with lambda = A^-1 dL/dalpha (one more PCG on the same symmetric matrix):
       dL/dz   = sum_j w_j [(t_j - E_j alpha) d(E_j lambda) - (E_j lambda) d(E_j alpha)] - reg d(lambda^T R alpha)
       dL/dt_j = w_j E_j lambda                                                     (the normal rows' targets)
-    The first line is a row functional with omega = c^lambda lambda + c^alpha alpha per row (nksr_feature_vjp); the
-    E_j alpha, E_j lambda are field evaluations at the constraint locations.  E itself is not kept."""
+    The first line is a row functional with omega = c^lambda lambda + c^alpha alpha per row (nksr_feature_vjp).  On the
+    assembled operator E_j alpha, E_j lambda are field evaluations at the constraint locations and E itself is not
+    kept.  On the matrix-free operator (KernelField._grad_operator) the kernel rows stay resident with the operator's
+    workspace until the backward: the adjoint PCG runs on the same operator and E_j alpha, E_j lambda are read from the
+    rows (nksr_op_constraint_values)."""
 
     @staticmethod
     def forward(ctx, field, args, normal_value, *z):
         pos_xyz, normal_xyz, pos_weight, normal_weight, reg_weight = args
+        ctx.matrix_free = field._grad_operator() == "matrix_free"
+        if ctx.matrix_free:
+            sysm = field.matrix_free_system(pos_xyz, normal_xyz, normal_value, pos_weight, normal_weight, reg_weight,
+                                            keep_constraints=True)
+            alpha = field._pcg_matrix_free(sysm, sysm.rhs)
+            ctx.field, ctx.sysm = field, sysm
+            ctx.save_for_backward(alpha)
+            return alpha
         sysm = field.assemble(pos_xyz, normal_xyz, normal_value, pos_weight, normal_weight, reg_weight,
                               keep_constraints=True)
         alpha = field._pcg(sysm, sysm.rhs)
@@ -729,29 +773,36 @@ class _KernelSolve(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_alpha):
-        field, sysm = ctx.field, ctx.sysm
+        field, sysm, mf = ctx.field, ctx.sysm, ctx.matrix_free
         (alpha,) = ctx.saved_tensors
         cons = sysm.cons
         tm = getattr(field, "_timer", None) or _lib.StageTimer(alpha.device, enabled=False)
         tm.mark("backward_start")
         g_alpha = g_alpha.detach().to(torch.float32).contiguous()
         if bool((g_alpha != 0).any()):
-            lam = field._pcg(sysm, g_alpha, adjoint=True)
+            lam = field._pcg_matrix_free(sysm, g_alpha, adjoint=True) if mf else field._pcg(sysm, g_alpha, adjoint=True)
         else:
             lam = torch.zeros_like(alpha)
             field.solve_info.update(adjoint_iterations=0, adjoint_relative_residual=0.0)
         n, C_ = sysm.n, field.channels
         dz = torch.zeros((n, C_), dtype=torch.float32, device=alpha.device)
         xs, base, ranges = cons.pos
-        f_a, _ = field._evaluate(alpha, xs, False)
-        f_l, _ = field._evaluate(lam, xs, False)
+        if mf:
+            vp, vn = field.constraint_values(sysm, alpha, lam)
+            f_a, f_l = vp[:, 0], vp[:, 1]
+        else:
+            f_a, _ = field._evaluate(alpha, xs, False)
+            f_l, _ = field._evaluate(lam, xs, False)
         coef = torch.stack([-cons.w_pos * f_a, -cons.w_pos * f_l], dim=1)         # omega = c^lam lam + c^alpha alpha
         field._feature_vjp(cons.pos, 0, coef, lam, alpha, dz)
         d_nv = None
         if cons.nrm is not None:
             xs_n = cons.nrm[0]
-            _, g_a = field._evaluate(alpha, xs_n, True)
-            _, g_l = field._evaluate(lam, xs_n, True)
+            if mf:
+                g_a, g_l = vn[:, 0], vn[:, 1]
+            else:
+                _, g_a = field._evaluate(alpha, xs_n, True)
+                _, g_l = field._evaluate(lam, xs_n, True)
             coef = torch.stack([cons.w_nrm * (cons.t_nrm - g_a), -cons.w_nrm * g_l], dim=1)     # (k, 2, 3)
             field._feature_vjp(cons.nrm, 1, coef, lam, alpha, dz)
             if ctx.needs_input_grad[2]:                                             # back to the caller's order

@@ -160,11 +160,15 @@ class TrainingScene:
         self.adaptive_depth = adaptive_depth
 
 
-def kernel_field(net, feat, dec_svh: SparseFeatureHierarchy, scene: TrainingScene, timer=None):
+def kernel_field(net, feat, dec_svh: SparseFeatureHierarchy, scene: TrainingScene, timer=None, operator=None):
     """the KernelField of models/nksr_net.py:91-112: basis features through the interpolators, position constraints at
     the input points, normal constraints (value -normal_features) at the voxel centres of the `adaptive_depth` finest
-    levels, solved with the solver weights of train.yaml.  Differentiable when grad is enabled (fields._KernelSolve)."""
+    levels, solved with the solver weights of train.yaml.  Differentiable when grad is enabled (fields._KernelSolve).
+    `operator` ('assembled' or 'matrix_free'), if given, sets field.solver_config['operator']: the matrix-free operator
+    runs the forward and the adjoint PCG without assembling the Gram matrix."""
     field = KernelField(dec_svh, net.interpolators, feat.basis_features)
+    if operator is not None:
+        field.solver_config["operator"] = operator
     if timer is not None:
         field._timer = timer
         timer.mark("solve_start")
@@ -230,18 +234,18 @@ def neural_field(net, feat, dec_svh: SparseFeatureHierarchy):
     return NeuralField(dec_svh, net.sdf_decoder, feat.basis_features, position_gradient=True)
 
 
-def kernel_losses(net, scene: TrainingScene, generator=None, feat=None, dec_svh=None, timer=None):
+def kernel_losses(net, scene: TrainingScene, generator=None, feat=None, dec_svh=None, timer=None, operator=None):
     """the field losses of a trainable NKSRNetwork on the scene: dict(total, gt_value, gt_normal, spatial, field), on
     the KernelField (kernel_field), or with geometry='neural' on the NeuralField (neural_field, no solve).  `feat`,
     `dec_svh`: an existing forward of the network (else one is run).  With volume ground truth (scene.gt) the dict
-    also holds spatial_empty, the empty-space term's share of spatial."""
+    also holds spatial_empty, the empty-space term's share of spatial.  `operator`: the kernel solve's (kernel_field)."""
     if feat is None:
         enc = net.encoder(scene.xyz, scene.normal, scene.enc_svh, 0)
         feat, dec_svh, _ = net.unet(enc, scene.enc_svh, adaptive_depth=scene.adaptive_depth)
     if getattr(net, "geometry", "kernel") == "neural":
         field = neural_field(net, feat, dec_svh)
     else:
-        field = kernel_field(net, feat, dec_svh, scene, timer)
+        field = kernel_field(net, feat, dec_svh, scene, timer, operator)
     l_val, l_nrm = gt_surface_loss(field, scene.ref_xyz, scene.ref_normal, generator=generator)
     extra = {}
     if scene.gt is None:
@@ -269,12 +273,12 @@ def use_predicted_structure(pd_structure_prob, generator=None):
     return bool(torch.rand((1,), generator=generator, device=dev).item() < p)
 
 
-def losses(net, scene: TrainingScene, generator=None, kernel=False, timer=None, pd_structure_prob=0.0):
+def losses(net, scene: TrainingScene, generator=None, kernel=False, timer=None, pd_structure_prob=0.0, operator=None):
     """forward of a trainable NKSRNetwork on the scene and its weighted losses: (total, structure, udf), and with
     `kernel` the kernel_losses dict as a fourth element (its total is included in the first).  The structure and UDF
     losses live on the third hierarchy unet() returns: the encoder hierarchy for structure='encoder', the grown one for
     structure='predicted' -- teacher-forced from the scene's ground truth, or grown from the prediction with
-    probability `pd_structure_prob`."""
+    probability `pd_structure_prob`.  `operator`: the kernel solve's (kernel_field)."""
     enc = net.encoder(scene.xyz, scene.normal, scene.enc_svh, 0)
     if getattr(net, "structure", "encoder") == "predicted":
         gt_dec = None if use_predicted_structure(pd_structure_prob, generator) else scene.gt_svh
@@ -289,7 +293,7 @@ def losses(net, scene: TrainingScene, generator=None, kernel=False, timer=None, 
     total = STRUCTURE_WEIGHT * l_struct + UDF_WEIGHT * l_udf
     if not kernel:
         return total, l_struct, l_udf
-    k = kernel_losses(net, scene, generator, feat, dec_svh, timer)
+    k = kernel_losses(net, scene, generator, feat, dec_svh, timer, operator)
     return total + k["total"], l_struct, l_udf, k
 
 
@@ -302,14 +306,15 @@ def make_optimizer(net):
 
 
 def train_step(net, opt, scene: TrainingScene, generator=None, marks=None, kernel=False, timer=None,
-               pd_structure_prob=0.0):
+               pd_structure_prob=0.0, operator=None):
     """one Adam step (gradient norm clipped to GRAD_CLIP); returns the (structure, udf) losses as tensors, and with
     `kernel` (the kernel-field losses added, trained through the kernel solve) a third element: the dict of the
     detached kernel losses.  `marks`, if given, is called with 'forward' / 'backward' / 'step' after each phase has
     been enqueued; `timer` (a StageTimer) receives the kernel solve's stage marks.  `pd_structure_prob`: see
-    `losses` (structure='predicted' only)."""
+    `losses` (structure='predicted' only).  `operator` ('assembled' or 'matrix_free'): the kernel solve's operator
+    (kernel_field); None keeps the field's own choice, which assembles for a grad-recording solve."""
     opt.zero_grad(set_to_none=True)
-    out = losses(net, scene, generator, kernel, timer, pd_structure_prob)
+    out = losses(net, scene, generator, kernel, timer, pd_structure_prob, operator)
     total, l_struct, l_udf = out[:3]
     if marks:
         marks("forward")

@@ -8,6 +8,7 @@ the structure and UDF losses (nksr_b200/training.py), Adam lr 1e-4, gradient nor
     python tools/train_unet.py --scene cfg4 --points 1000000 --depth 4 --udf --steps 10
     python tools/train_unet.py --scene sphere --points 200000 --depth 4 --geometry neural --steps 30
     python tools/train_unet.py --scene cfg4 --points 1000000 --depth 4 --kernel-losses --vol-sup --steps 10
+    python tools/train_unet.py --scene cfg4 --points 1000000 --depth 4 --kernel-losses --operator matrix_free --steps 10
 
 Scenes: 'sphere' (tests/clouds.py, exact normals) or 'cfg4' (a crop of bench.py's outdoor scene at its own density,
 normals from the kNN preprocess).  Every step prints one JSON line: the losses and the CUDA-event times of the forward,
@@ -16,7 +17,8 @@ step.  The last line is a summary over the steps after the first two: median tim
 achieved TFLOP/s (2 nnz_taps c_in c_out per call) and GB/s per (c_in, c_out) shape, and the GPU's name and power limit.
 --kernel-losses adds the kernel-field losses (GT-surface value / normal, spatial TSDF), trained through the kernel solve,
 and reports them per step with the CUDA-event times of the forward solve (assembly + PCG), the adjoint PCG and the VJP
-kernels (with the field evaluations they need).
+kernels (with the field evaluations they need).  --operator matrix_free runs both PCGs on the matrix-free operator
+(no Gram matrix); the solve time then sums the kernel rows, the operator setup and the PCG.
 --structure predicted grows the decoder hierarchy from the structure head (teacher-forced from the ground truth, or
 from the prediction with probability --pd-structure-prob); after training one more line reports, per level, the
 structure accuracy and the sizes |E_l| (encoder), |T_l| (grown) and |dec_l| (kept), the CUDA-event time of every growth
@@ -202,6 +204,8 @@ def main(argv=None):
                     help="udf.enabled: the UDF loss on the NeuralField over every level (DESIGN.md SPEC S17)")
     ap.add_argument("--vol-sup", action="store_true",
                     help="cfg4: volume ground truth from the sensor rays (DESIGN.md SPEC S19)")
+    ap.add_argument("--operator", choices=("assembled", "matrix_free"), default=None,
+                    help="--kernel-losses: the kernel solve's operator (default: assembled)")
     ap.add_argument("--geometry", choices=("kernel", "neural"), default="kernel",
                     help="output field: the kernel solve, or the NeuralField sdf_decoder(u(x)) (implies --kernel-losses)")
     args = ap.parse_args(argv)
@@ -230,7 +234,7 @@ def main(argv=None):
     timer = KernelTimer(U)
     info = dict(gpu_info(0), scene=args.scene, points=int(scene.xyz.shape[0]), voxel_size=scene.voxel_size,
                 depth=args.depth, precision=args.precision, structure=args.structure,
-                pd_structure_prob=args.pd_structure_prob, udf=args.udf, geometry=args.geometry,
+                pd_structure_prob=args.pd_structure_prob, udf=args.udf, geometry=args.geometry, operator=args.operator,
                 voxels=[scene.enc_svh.num_voxels(l) for l in range(args.depth)])
     if vol is not None:
         info["volume"] = vol
@@ -248,7 +252,7 @@ def main(argv=None):
         timer.phase = "forward"
         stages = StageTimer(dev, enabled=True) if args.kernel_losses else None
         out = T.train_step(net, opt, scene, gen, marks, kernel=args.kernel_losses, timer=stages,
-                           pd_structure_prob=args.pd_structure_prob)
+                           pd_structure_prob=args.pd_structure_prob, operator=args.operator)
         l_struct, l_udf = out[:2]
         timer.phase = "forward"
         torch.cuda.synchronize()
@@ -258,7 +262,7 @@ def main(argv=None):
             st = stages.report()
             kern = {name: round(float(v), 6) for name, v in out[2].items()}
             kern.update(kernel_solve_ms=round(sum(st.get(s, 0.0) for s in ("kernel_rows", "gram_count", "gram_blocks",
-                                                                           "gram_fill", "pcg")), 3),
+                                                                           "gram_fill", "operator_setup", "pcg")), 3),
                         adjoint_pcg_ms=round(st.get("adjoint_pcg", 0.0), 3),
                         vjp_ms=round(st.get("feature_vjp", 0.0) + st.get("evaluate_vjp", 0.0), 3))
         row = dict(step=step, structure=round(float(l_struct), 6), udf=round(float(l_udf), 6), **kern,
