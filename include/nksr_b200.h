@@ -549,6 +549,31 @@ NKSR_API size_t nksr_tsdf_volume_workspace_bytes(const int64_t* dims3);
 NKSR_API int nksr_tsdf_volume(const float* xyz, const float* sensor, int64_t n, const float* volume_min3, float h,
                               const int64_t* dims3, float tau, float* volume, void* ws, size_t ws_bytes, void* stream);
 
+/* ---- mesh occupancy by ray parity ('o3d-iou' of metrics.MeshEvaluator, metrics.py:180-188; DESIGN.md SPEC S20).
+ * Mesh v: float[V*3], f: int32[n_tri*3] (indices in [0, V), any winding, degenerate and duplicate triangles allowed).
+ * Build (an LBVH, one triangle per leaf):
+ *   nksr_bvh_keys: scene (device float[8]) = centroid box lo xyz, hi xyz, max |vertex coordinate|, -;
+ *     keys (int64[n_tri]) = 63-bit Morton codes of the centroids in that box, idx (int32[n_tri]) = 0..n_tri-1;
+ *   the caller sorts (keys, idx) with nksr_sort_pairs;
+ *   nksr_bvh_hierarchy: the sorted keys -> nodes (float[16 * (n_tri - 1)]: per internal node the two child boxes and
+ *     child codes) and the parent table in ws (ws: nksr_bvh_workspace_bytes(n_tri) bytes, kept for the refit);
+ *   nksr_bvh_refit: the sorted idx -> tris (float[12 * n_tri], the triangles in leaf order) and the child boxes.
+ * n_tri = 1 needs no nodes (nullable) and no hierarchy call.
+ * nksr_mesh_occupancy: inside[i] (uint8[m]) = 1 iff more than k/2 of the k rays from query[i] (float[m*3]) cross the
+ * mesh an odd number of times; dirs = device float[k*3] (every component nonzero) or NULL for the first k built-in
+ * directions; k odd, 1 <= k <= 9.  Equal bit for bit to testing every triangle (the box test is conservative);
+ * n_tri = 0 gives all 0. */
+NKSR_API size_t nksr_bvh_workspace_bytes(int64_t n_tri);
+NKSR_API int nksr_bvh_keys(const float* v, const int32_t* f, int64_t n_tri, float* scene, int64_t* keys, int32_t* idx,
+                           void* stream);
+NKSR_API int nksr_bvh_hierarchy(const int64_t* keys, int64_t n_tri, float* nodes, void* ws, size_t ws_bytes,
+                                void* stream);
+NKSR_API int nksr_bvh_refit(const float* v, const int32_t* f, const int32_t* idx, int64_t n_tri, float* nodes,
+                            float* tris, void* ws, size_t ws_bytes, void* stream);
+NKSR_API int nksr_mesh_occupancy(const float* nodes, const float* tris, const float* scene, int64_t n_tri,
+                                 const float* query, int64_t m, const float* dirs, int k, uint8_t* inside,
+                                 void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -148,6 +148,11 @@ _SIGNATURES = {
     "nksr_metric_nearest": ("i", "Spppp" + "qppqpi" + "pppppp"),
     "nksr_tsdf_volume_workspace_bytes": ("z", "p"),
     "nksr_tsdf_volume": ("i", "ppqpfpfppzp"),
+    "nksr_bvh_workspace_bytes": ("z", "q"),
+    "nksr_bvh_keys": ("i", "ppqpppp"),
+    "nksr_bvh_hierarchy": ("i", "pqppzp"),
+    "nksr_bvh_refit": ("i", "pppqpppzp"),
+    "nksr_mesh_occupancy": ("i", "pppqpqpipp"),
 }
 
 _lib = None

@@ -7,6 +7,10 @@ Reference contract:
 The mesh is sampled area-uniformly (csrc/metrics.cu: k_sample_surface) and both nearest-neighbour passes are exact
 (k_metric_nearest on the multi-level voxel hash, k_metric_far for the queries the hierarchy does not resolve); the
 means and threshold fractions are fp64 reductions in torch.  DESIGN.md SPEC S18 defines every step.
+
+`o3d-iou` (opt-in, MeshEvaluator(occupancy_rays=K)) is the volumetric IoU of the reference's ONet occupancy samples
+against MeshOccupancy, a ray-parity occupancy of the mesh on an LBVH (csrc/raycast.cu; SPEC S20).  The reference takes
+its occupancy from a package outside its tree, so the value is this project's rule, not a reproduction.
 """
 from __future__ import annotations
 
@@ -18,12 +22,13 @@ from typing import Optional
 import numpy as np
 import torch
 
-from ._lib import MAX_DEPTH, NksrError, call, require_cuda, stream_ptr
+from ._lib import MAX_DEPTH, NksrError, _ws, call, require_cuda, sort_pairs, stream_ptr
 
 _log = logging.getLogger(__name__)
 
 THRESHOLDS = (0.01, 0.015, 0.02, 0.002, 0.1)
 START_LEVEL = 2         # first level of the nearest-point search, as for PCNNField
+MAX_RAYS = 9            # KMAX of SPEC S20: the number of built-in ray directions (csrc/raycast.cu)
 _NAN = float("nan")
 
 
@@ -118,6 +123,88 @@ def summarise(completeness: torch.Tensor, completeness_dot: torch.Tensor, accura
     }
 
 
+def _check_rays(k) -> int:
+    k = int(k)
+    if k < 1 or k > MAX_RAYS or k % 2 == 0:
+        raise ValueError(f"the number of rays must be odd and in [1, {MAX_RAYS}], got {k}")
+    return k
+
+
+class MeshOccupancy:
+    """Inside / outside of a triangle mesh by ray parity (SPEC S20): a query is inside when more than half of its K
+    rays cross the mesh an odd number of times.  Winding never enters, so triangle soups and mixed orientations are
+    fine; on a closed mesh every ray agrees, on an open one the vote is a definition.  The BVH is built once here;
+    `contains` answers any number of query batches.  CUDA only."""
+
+    def __init__(self, v: torch.Tensor, f: torch.Tensor):
+        require_cuda(v, "v")
+        require_cuda(f, "f")
+        dev = v.device
+        v = v.detach().to(torch.float32).reshape(-1, 3).contiguous()
+        f = f.detach().to(dev).reshape(-1, 3)
+        n_v, t = v.shape[0], f.shape[0]
+        if t >= 2 ** 31:
+            raise NksrError(f"{t} triangles: the occupancy BVH holds fewer than 2^31")
+        if t and (int(f.min()) < 0 or int(f.max()) >= n_v):
+            raise NksrError(f"face indices must lie in [0, {n_v})")
+        if not bool(torch.isfinite(v).all()):
+            raise NksrError("mesh vertices must be finite")
+        f = f.to(torch.int32).contiguous()
+        self.device, self.n_tri = dev, t
+        self.scene = torch.zeros(8, dtype=torch.float32, device=dev)
+        self.nodes = torch.empty((max(t - 1, 0), 16), dtype=torch.float32, device=dev)
+        self.tris = torch.empty((t, 12), dtype=torch.float32, device=dev)
+        if t == 0:
+            return
+        st = stream_ptr(dev)
+        keys = torch.empty(t, dtype=torch.int64, device=dev)
+        idx = torch.empty(t, dtype=torch.int32, device=dev)
+        call("nksr_bvh_keys", v, f, t, self.scene, keys, idx, st)
+        keys, idx = sort_pairs(keys, idx)
+        nb = call("nksr_bvh_workspace_bytes", t)
+        ws = _ws(nb, dev)
+        if t > 1:
+            call("nksr_bvh_hierarchy", keys, t, self.nodes, ws, nb, st)
+        call("nksr_bvh_refit", v, f, idx, t, self.nodes if t > 1 else None, self.tris, ws, nb, st)
+
+    def contains(self, points, n_rays: int = 3) -> torch.Tensor:
+        """bool (m,): inside by the vote of the first n_rays built-in directions (odd, 1 <= n_rays <= 9)"""
+        return occupancy_along(self, points, None, _check_rays(n_rays))
+
+    def __repr__(self):
+        return f"MeshOccupancy(triangles={self.n_tri}, device={self.device})"
+
+
+def occupancy_along(occ: MeshOccupancy, points, directions=None, n_rays: Optional[int] = None) -> torch.Tensor:
+    """MeshOccupancy.contains with explicit ray directions ((K, 3), K odd in [1, 9], every component nonzero and
+    finite) or, with directions None, the first n_rays built-in ones"""
+    if isinstance(points, torch.Tensor):
+        require_cuda(points, "points")
+    q = _as_tensor(points, occ.device, torch.float32).reshape(-1, 3)
+    if not bool(torch.isfinite(q).all()):
+        raise NksrError("query points must be finite")
+    dirs = None
+    if directions is not None:
+        dirs = _as_tensor(directions, occ.device, torch.float32).reshape(-1, 3)
+        k = _check_rays(dirs.shape[0])
+        if not bool((torch.isfinite(dirs) & (dirs != 0)).all()):
+            raise ValueError("every ray direction component must be finite and nonzero")
+    else:
+        k = _check_rays(n_rays)
+    m = q.shape[0]
+    inside = torch.empty(m, dtype=torch.uint8, device=occ.device)
+    if m:
+        call("nksr_mesh_occupancy", occ.nodes if occ.n_tri > 1 else None, occ.tris, occ.scene, occ.n_tri, q, m, dirs,
+             k, inside, stream_ptr(occ.device))
+    return inside.bool()
+
+
+def occupancy_iou(pred: torch.Tensor, gt: torch.Tensor) -> float:
+    """the reference's volumetric IoU: |pred & gt| / (|pred | gt| + 1e-6), integer counts, fp64 division"""
+    both = torch.stack([(pred & gt).sum(), (pred | gt).sum()]).tolist()
+    return float(both[0]) / (float(both[1]) + 1e-6)
+
+
 METRIC_KEYS = ("completeness", "accuracy", "normals completeness", "normals accuracy", "normals", "completeness2",
                "accuracy2", "chamfer-L2", "chamfer-L1", "f-precision", "f-recall", "f-score", "f-score-15",
                "f-score-20", "f-precision-outdoor", "f-recall-outdoor", "f-score-outdoor")
@@ -136,20 +223,24 @@ def mesh_arrays(mesh):
 
 class MeshEvaluator:
     """Drop-in for the reference's metrics.MeshEvaluator: same constructor, class attributes, methods, keys and
-    definitions; CUDA only.  `o3d-iou` (a mesh-occupancy IoU on ray queries the reference takes from a package
-    outside its tree) is not provided."""
+    definitions; CUDA only.  `o3d-iou` (the volumetric IoU on the ONet occupancy samples) is computed only when
+    `occupancy_rays` (odd, 1..9) is given: it uses this project's ray-parity rule (MeshOccupancy, SPEC S20), not the
+    package the reference takes it from, so a caller opts in knowingly."""
 
     ESSENTIAL_METRICS = ["chamfer-L1", "f-score", "normals"]
     ALL_METRICS = ["completeness", "accuracy", "normals completeness", "normals accuracy", "normals",
                    "completeness2", "accuracy2", "chamfer-L2",
                    "chamfer-L1", "f-precision", "f-recall", "f-score", "f-score-15", "f-score-20"]
 
-    def __init__(self, n_points=100000, metric_names=ALL_METRICS, device=None, seed: int = 0):
+    def __init__(self, n_points=100000, metric_names=ALL_METRICS, device=None, seed: int = 0,
+                 occupancy_rays: Optional[int] = None):
         names = list(metric_names)
-        if "o3d-iou" in names:
-            raise ValueError("'o3d-iou' is not provided: it needs a ray-distance occupancy query of the mesh that the "
-                             "reference takes from a package outside its tree")
-        unknown = [k for k in names if k not in METRIC_KEYS]
+        if occupancy_rays is not None:
+            occupancy_rays = _check_rays(occupancy_rays)
+        elif "o3d-iou" in names:
+            raise ValueError("'o3d-iou' needs occupancy_rays=K (odd, 1..9): its mesh occupancy is this project's "
+                             "ray-parity rule (SPEC S20), not the package the reference takes it from")
+        unknown = [k for k in names if k not in METRIC_KEYS and not (k == "o3d-iou" and occupancy_rays)]
         if unknown:
             raise ValueError(f"unknown metric names {unknown}; known: {list(METRIC_KEYS)}")
         self.n_points = int(n_points)
@@ -158,6 +249,7 @@ class MeshEvaluator:
         self.metric_names = names
         self.device = torch.device(device) if device is not None else None
         self.seed = int(seed)
+        self.occupancy_rays = occupancy_rays
 
     def _device_for(self, a) -> torch.device:
         if self.device is not None:
@@ -173,10 +265,13 @@ class MeshEvaluator:
         v = _as_tensor(v, dev, torch.float32).reshape(-1, 3)
         f = _as_tensor(f, dev, torch.int32).reshape(-1, 3)
         xyz, nrm, _ = sample_surface(v, f, self.n_points, self.seed)
-        return self._evaluate(xyz, pointcloud_tgt, nrm, normals_tgt, onet_samples, mesh)
+        return self._evaluate(xyz, pointcloud_tgt, nrm, normals_tgt, onet_samples, (v, f))
 
     def _evaluate(self, pointcloud, pointcloud_tgt, normals=None, normals_tgt=None, onet_samples=None, mesh=None):
         dev = self._device_for(pointcloud)
+        want_iou = "o3d-iou" in self.metric_names
+        if want_iou and (onet_samples is None or mesh is None):
+            raise ValueError("'o3d-iou' needs the mesh and onet_samples = (points (N, 3), occupancy (N,))")
         if int(pointcloud.shape[0]) == 0:
             _log.warning("Empty pointcloud / mesh detected! Return NaN metric!")
             return {k: _NAN for k in self.metric_names}
@@ -189,7 +284,26 @@ class MeshEvaluator:
         comp, _, comp_dot = nearest_neighbours(tgt, pts, nrm_t, nrm)
         acc, _, acc_dot = nearest_neighbours(pts, tgt, nrm, nrm_t)
         out = summarise(comp, comp_dot, acc, acc_dot, tuple(self.thresholds.tolist()))
+        if want_iou:
+            out["o3d-iou"] = self._occupancy_iou(mesh, onet_samples, dev)
         return {k: out[k] for k in self.metric_names}
 
+    def _occupancy_iou(self, mesh, onet_samples, dev) -> float:
+        """o3d-iou of the reference (metrics.py:180-188): occupancy of onet_samples[0] against onet_samples[1] != 0"""
+        v, f = mesh_arrays(mesh)
+        v = _as_tensor(v, dev, torch.float32).reshape(-1, 3)
+        f = _as_tensor(f, dev, torch.int64).reshape(-1, 3)
+        if f.shape[0] == 0:
+            return _NAN
+        pts = _as_tensor(onet_samples[0], dev, torch.float32).reshape(-1, 3)
+        gt = onet_samples[1]
+        gt = (gt.detach().to(dev) if isinstance(gt, torch.Tensor) else torch.from_numpy(np.asarray(gt)).to(dev))
+        gt = gt.reshape(-1) != 0
+        if gt.shape[0] != pts.shape[0]:
+            raise ValueError(f"onet_samples: {pts.shape[0]} points but {gt.shape[0]} occupancy values")
+        pred = MeshOccupancy(v, f).contains(pts, self.occupancy_rays)
+        return occupancy_iou(pred, gt)
 
-__all__ = ["MeshEvaluator", "sample_surface", "nearest_neighbours", "summarise", "mesh_arrays", "THRESHOLDS"]
+
+__all__ = ["MeshEvaluator", "MeshOccupancy", "sample_surface", "nearest_neighbours", "summarise", "mesh_arrays",
+           "occupancy_iou", "THRESHOLDS", "MAX_RAYS"]
