@@ -557,12 +557,17 @@ NKSR_API int nksr_tsdf_volume(const float* xyz, const float* sensor, int64_t n, 
  *   the caller sorts (keys, idx) with nksr_sort_pairs;
  *   nksr_bvh_hierarchy: the sorted keys -> nodes (float[16 * (n_tri - 1)]: per internal node the two child boxes and
  *     child codes) and the parent table in ws (ws: nksr_bvh_workspace_bytes(n_tri) bytes, kept for the refit);
- *   nksr_bvh_refit: the sorted idx -> tris (float[12 * n_tri], the triangles in leaf order) and the child boxes.
+ *   nksr_bvh_refit: the sorted idx -> tris (float[12 * n_tri], the triangles in leaf order, the original triangle
+ *     index as the int32 bits of each leaf's word 3) and the child boxes.
  * n_tri = 1 needs no nodes (nullable) and no hierarchy call.
  * nksr_mesh_occupancy: inside[i] (uint8[m]) = 1 iff more than k/2 of the k rays from query[i] (float[m*3]) cross the
  * mesh an odd number of times; dirs = device float[k*3] (every component nonzero) or NULL for the first k built-in
  * directions; k odd, 1 <= k <= 9.  Equal bit for bit to testing every triangle (the box test is conservative);
- * n_tri = 0 gives all 0. */
+ * n_tri = 0 gives all 0.
+ * nksr_mesh_closest (SPEC S21): for every query[i] (float[m*3], finite) the closest triangle of the mesh on the same
+ * BVH: dist[i] (float[m]) = sqrt(d2), point[i] (float[m*3]) = the closest point whose d2 that is, tri[i] (int32[m]) =
+ * the original triangle index; equal d2 go to the lower index.  Equal bit for bit to testing every triangle (the box
+ * bound is conservative); n_tri = 0 gives dist inf, point NaN, tri -1. */
 NKSR_API size_t nksr_bvh_workspace_bytes(int64_t n_tri);
 NKSR_API int nksr_bvh_keys(const float* v, const int32_t* f, int64_t n_tri, float* scene, int64_t* keys, int32_t* idx,
                            void* stream);
@@ -573,6 +578,8 @@ NKSR_API int nksr_bvh_refit(const float* v, const int32_t* f, const int32_t* idx
 NKSR_API int nksr_mesh_occupancy(const float* nodes, const float* tris, const float* scene, int64_t n_tri,
                                  const float* query, int64_t m, const float* dirs, int k, uint8_t* inside,
                                  void* stream);
+NKSR_API int nksr_mesh_closest(const float* nodes, const float* tris, const float* scene, int64_t n_tri,
+                               const float* query, int64_t m, float* dist, float* point, int32_t* tri, void* stream);
 
 #ifdef __cplusplus
 }

@@ -153,6 +153,7 @@ _SIGNATURES = {
     "nksr_bvh_hierarchy": ("i", "pqppzp"),
     "nksr_bvh_refit": ("i", "pppqpppzp"),
     "nksr_mesh_occupancy": ("i", "pppqpqpipp"),
+    "nksr_mesh_closest": ("i", "pppqpqpppp"),
 }
 
 _lib = None

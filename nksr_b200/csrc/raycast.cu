@@ -13,7 +13,13 @@
 // inflates its far distance as in Ize, "Robust BVH Ray Traversal" (JCGT 2013).  So the count, and the occupancy, is
 // the brute-force rule's bit for bit.
 //
-// Built with --fmad=false: the rule rounds every fp32 and fp64 product and sum on its own (SPEC S20).
+// Distance: k_mesh_closest, one thread per query, best-first over the same LBVH (nearer child first, the farther one
+// pushed with its bound).  SPEC S21's point-triangle routine gives each triangle's closest point; a child box is
+// skipped only when its padded lower bound is strictly above the best squared distance so far, and the bound never
+// exceeds the routine's d2 of any triangle inside, so the answer, ties to the lower original index included, is the
+// brute force's bit for bit.
+//
+// Built with --fmad=false: the rules round every fp32 and fp64 product and sum on their own (SPEC S20, S21).
 #include "common.cuh"
 
 namespace {
@@ -203,13 +209,15 @@ k_bvh_refit(const float* __restrict__ v, const int32_t* __restrict__ f, const in
   const int64_t j = blockIdx.x * (int64_t)kBvhThreads + threadIdx.x;
   if (j >= n) return;
   float p[3][3];
-  load_tri(v, f, __ldg(idx + j), p);
+  const int32_t orig = __ldg(idx + j);
+  load_tri(v, f, orig, p);
   // SPEC S20 tests the vertices in lexicographic (x, y, z) order, so neither the winding nor the rotation of a
   // triangle changes how its sums are rounded
   if (lex_less(p[1], p[0])) swap3(p[0], p[1]);
   if (lex_less(p[2], p[1])) swap3(p[1], p[2]);
   if (lex_less(p[1], p[0])) swap3(p[0], p[1]);
-  tris[3 * j] = make_float4(p[0][0], p[0][1], p[0][2], 0.f);
+  // the first vertex's .w carries the original triangle index, which the distance query reports and breaks ties on
+  tris[3 * j] = make_float4(p[0][0], p[0][1], p[0][2], __int_as_float(orig));
   tris[3 * j + 1] = make_float4(p[1][0], p[1][1], p[1][2], 0.f);
   tris[3 * j + 2] = make_float4(p[2][0], p[2][1], p[2][2], 0.f);
   if (n == 1) return;
@@ -362,6 +370,183 @@ k_mesh_occupancy(const float4* __restrict__ nodes, const float4* __restrict__ tr
   inside[i] = 2 * votes > k_rays;
 }
 
+// ---- SPEC S21: the closest point of a triangle.  Every product, sum and difference is rounded on its own (the file
+// is built with --fmad=false), dots are ((x x' + y y') + z z'), divisions and the square root are correctly rounded.
+
+constexpr int kDistThreads = 128;
+
+__device__ __forceinline__ float dot3(const float a[3], const float b[3]) {
+  return (a[0] * b[0] + a[1] * b[1]) + a[2] * b[2];
+}
+
+__device__ __forceinline__ void cross3(const float a[3], const float b[3], float c[3]) {
+  c[0] = a[1] * b[2] - a[2] * b[1];
+  c[1] = a[2] * b[0] - a[0] * b[2];
+  c[2] = a[0] * b[1] - a[1] * b[0];
+}
+
+__device__ __forceinline__ float dist2(const float p[3], const float c[3]) {
+  const float dx = p[0] - c[0], dy = p[1] - c[1], dz = p[2] - c[2];
+  return (dx * dx + dy * dy) + dz * dz;
+}
+
+// candidate on segment (P, Q): P when e.(p - P) <= 0 (a zero-length edge included), Q when it reaches e.e, else
+// P + t e with t = e.(p - P) / e.e; it replaces the best one only when its d2 is strictly smaller
+__device__ __forceinline__ void closest_on_segment(const float P[3], const float Q[3], const float p[3], float& best,
+                                                   float x[3]) {
+  float e[3], ap[3], c[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    e[k] = Q[k] - P[k];
+    ap[k] = p[k] - P[k];
+  }
+  const float num = dot3(e, ap), den = dot3(e, e);
+  if (!(num > 0.f)) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) c[k] = P[k];
+  } else if (num >= den) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) c[k] = Q[k];
+  } else {
+    const float t = __fdiv_rn(num, den);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) c[k] = P[k] + t * e[k];
+  }
+  const float d2 = dist2(p, c);
+  if (d2 < best) {
+    best = d2;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) x[k] = c[k];
+  }
+}
+
+// SPEC S21 for the lexicographically sorted vertices a <= b <= c: the face candidate (when the projection's scaled
+// barycentric weights va = n.(bp x cp), vb = n.(cp x ap), vc = n.(ap x bp), n = ab x ac, are all >= 0 and their sum is
+// positive and finite), then the segments ab, ac, bc;
+// the smallest d2 wins, the earlier candidate on ties.  Returns d2 and the point in x.
+__device__ __forceinline__ float closest_on_triangle(const float a[3], const float b[3], const float c[3],
+                                                     const float p[3], float x[3]) {
+  float ab[3], ac[3], ap[3], bp[3], cp[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    ab[k] = b[k] - a[k];
+    ac[k] = c[k] - a[k];
+    ap[k] = p[k] - a[k];
+    bp[k] = p[k] - b[k];
+    cp[k] = p[k] - c[k];
+  }
+  float n[3], s[3];
+  cross3(ab, ac, n);
+  cross3(bp, cp, s);
+  const float va = dot3(n, s);
+  cross3(cp, ap, s);
+  const float vb = dot3(n, s);
+  cross3(ap, bp, s);
+  const float vc = dot3(n, s);
+  float best = INFINITY;
+  if (va >= 0.f && vb >= 0.f && vc >= 0.f) {
+    const float den = (va + vb) + vc;
+    if (den > 0.f && den < INFINITY) {
+      const float v = __fdiv_rn(vb, den), w = __fdiv_rn(vc, den);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) x[k] = (a[k] + v * ab[k]) + w * ac[k];
+      best = dist2(p, x);
+    }
+  }
+  closest_on_segment(a, b, p, best, x);
+  closest_on_segment(a, c, p, best, x);
+  closest_on_segment(b, c, p, best, x);
+  return best;
+}
+
+// squared distance from p to the box padded by pad on every side, each gap and sum rounded; never above the d2 that
+// closest_on_triangle reports for a triangle inside the unpadded box (DESIGN.md section 4.7)
+__device__ __forceinline__ float box_bound(const float4 lo, const float4 hi, const float pad, const float p[3]) {
+  const float gx = fmaxf(fmaxf((lo.x - pad) - p[0], p[0] - (hi.x + pad)), 0.f);
+  const float gy = fmaxf(fmaxf((lo.y - pad) - p[1], p[1] - (hi.y + pad)), 0.f);
+  const float gz = fmaxf(fmaxf((lo.z - pad) - p[2], p[2] - (hi.z + pad)), 0.f);
+  return (gx * gx + gy * gy) + gz * gz;
+}
+
+struct Best {
+  float d2;
+  int32_t tri;
+  float x[3];
+};
+
+// the leaf-order triangle j against the best so far: smaller d2, or equal d2 and a lower original index, wins
+__device__ __forceinline__ void test_leaf(const float4* __restrict__ tris, const int32_t j, const float p[3],
+                                          Best& best) {
+  const float4 wa = __ldg(tris + 3 * (int64_t)j), wb = __ldg(tris + 3 * (int64_t)j + 1),
+               wc = __ldg(tris + 3 * (int64_t)j + 2);
+  const float a[3] = {wa.x, wa.y, wa.z}, b[3] = {wb.x, wb.y, wb.z}, c[3] = {wc.x, wc.y, wc.z};
+  float x[3];
+  const float d2 = closest_on_triangle(a, b, c, p, x);
+  const int32_t t = __float_as_int(wa.w);
+  if (d2 < best.d2 || (d2 == best.d2 && t < best.tri)) {
+    best.d2 = d2;
+    best.tri = t;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) best.x[k] = x[k];
+  }
+}
+
+__global__ void __launch_bounds__(kDistThreads)
+k_mesh_closest(const float4* __restrict__ nodes, const float4* __restrict__ tris, const float* __restrict__ scene,
+               const int64_t n_tri, const float* __restrict__ query, const int64_t m, float* __restrict__ dist,
+               float* __restrict__ point, int32_t* __restrict__ tri) {
+  const int64_t i = blockIdx.x * (int64_t)kDistThreads + threadIdx.x;
+  if (i >= m) return;
+  Best best = {INFINITY, INT32_MAX, {NAN, NAN, NAN}};
+  if (n_tri > 0) {
+    const float p[3] = {__ldg(query + 3 * i), __ldg(query + 3 * i + 1), __ldg(query + 3 * i + 2)};
+    if (n_tri == 1) {
+      test_leaf(tris, 0, p, best);
+    } else {
+      // every rounding of a candidate point stays within 2^-18 (M + |q|_inf) of the triangle's box (section 4.7)
+      const float pad = (__ldg(scene + 6) + fmaxf(fabsf(p[0]), fmaxf(fabsf(p[1]), fabsf(p[2])))) * 0x1p-18f;
+      int32_t stack[kStack];
+      float stack_bound[kStack];
+      int sp = 0;
+      int32_t node = 0;
+      for (;;) {
+        const float4* nd = nodes + 4 * (int64_t)node;
+        const float4 a = __ldg(nd), b = __ldg(nd + 1), c = __ldg(nd + 2), e = __ldg(nd + 3);
+        const float lb0 = box_bound(a, b, pad, p), lb1 = box_bound(c, e, pad, p);
+        const bool swap = lb1 < lb0;     // nearer child first, child 0 on equal bounds
+        const int32_t near = __float_as_int(swap ? b.w : a.w), far = __float_as_int(swap ? a.w : b.w);
+        const float near_lb = swap ? lb1 : lb0, far_lb = swap ? lb0 : lb1;
+        int32_t next = -1;
+        if (!(near_lb > best.d2)) {
+          if (near < 0) test_leaf(tris, ~near, p, best);
+          else next = near;
+        }
+        if (!(far_lb > best.d2)) {
+          if (far < 0) {
+            test_leaf(tris, ~far, p, best);
+          } else if (next < 0) {
+            next = far;
+          } else {
+            stack[sp] = far;
+            stack_bound[sp++] = far_lb;
+          }
+        }
+        while (next < 0 && sp > 0) {
+          --sp;
+          if (!(stack_bound[sp] > best.d2)) next = stack[sp];
+        }
+        if (next < 0) break;
+        node = next;
+      }
+    }
+  }
+  dist[i] = __fsqrt_rn(best.d2);
+  point[3 * i] = best.x[0];
+  point[3 * i + 1] = best.x[1];
+  point[3 * i + 2] = best.x[2];
+  tri[i] = n_tri > 0 ? best.tri : -1;
+}
+
 }  // namespace
 
 extern "C" {
@@ -430,6 +615,19 @@ int nksr_mesh_occupancy(const float* nodes, const float* tris, const float* scen
   k_mesh_occupancy<<<grid_for(m, kOccThreads), kOccThreads, 0, st>>>(
       reinterpret_cast<const float4*>(nodes), reinterpret_cast<const float4*>(tris), scene, n_tri, query, m, dirs,
       k_rays, inside);
+  NKSR_CHECK_LAUNCH();
+  return NKSR_OK;
+}
+
+int nksr_mesh_closest(const float* nodes, const float* tris, const float* scene, int64_t n_tri, const float* query,
+                      int64_t m, float* dist, float* point, int32_t* tri, void* stream) {
+  if (n_tri < 0 || n_tri > INT32_MAX || m < 0) return NKSR_E_INVALID;
+  if (m == 0) return NKSR_OK;
+  if (!query || !dist || !point || !tri) return NKSR_E_INVALID;
+  if (n_tri > 0 && (!tris || !scene || (n_tri > 1 && !nodes))) return NKSR_E_INVALID;
+  k_mesh_closest<<<grid_for(m, kDistThreads), kDistThreads, 0, as_stream(stream)>>>(
+      reinterpret_cast<const float4*>(nodes), reinterpret_cast<const float4*>(tris), scene, n_tri, query, m, dist,
+      point, tri);
   NKSR_CHECK_LAUNCH();
   return NKSR_OK;
 }

@@ -9,6 +9,12 @@ supervision its default configs train with (configs/default/train.yaml: supervis
 
 The reference ships such volumes as data only; `from_sensor_rays` builds one from a LiDAR-like cloud whose points
 carry their sensor position.
+
+Mesh ground truth for object datasets (a closed mesh such as ShapeNet's), SPEC S21:
+
+    gt = MeshGroundTruth(v, f, tau)                       # the BVH of metrics.MeshOccupancy, surface samples
+    sdf = gt.query_sdf(q)                                 # -signed_distance: positive inside
+    cls = gt.query_classification(q)                      # 1 outside with |sdf| >= band tau, else 0
 """
 from __future__ import annotations
 
@@ -20,6 +26,7 @@ import torch.nn.functional as F
 
 from . import _lib
 from ._lib import call, stream_ptr
+from .metrics import MeshOccupancy, _check_rays, sample_surface
 from .sdfgen import sdf_from_points
 
 _NODE_BYTES = 4 + 8       # the fp32 volume and the builder's 64-bit key per node
@@ -139,3 +146,51 @@ class PointTSDFVolume:
         near = fin & (v.abs() < 1.0)
         n = max(v.numel(), 1)
         return dict(near=float(near.sum()) / n, free=float((fin & ~near).sum()) / n, unknown=float((~fin).sum()) / n)
+
+
+class MeshGroundTruth:
+    """exact SDF supervision from a triangle mesh (SPEC S21), with the three methods TrainingScene and the losses use.
+    The surface samples are `n_surface` area-uniform points of sample_surface with their unit triangle normals
+    (oriented by the winding); the SDF is the distance to the closest triangle on the BVH, signed by the ray-parity
+    occupancy of `n_rays` rays (SPEC S20), so the sign is right on a closed mesh whatever its winding.  `tau` is the
+    truncation that separates near-surface from empty space in query_classification.  The losses ask query_sdf and
+    query_classification about the same samples, so the last query tensor's (distance, inside) is kept and reused
+    while that tensor is unchanged (same object, same in-place version counter)."""
+
+    def __init__(self, v: torch.Tensor, f: torch.Tensor, tau: float, n_surface: int = 100_000, n_rays: int = 3,
+                 seed: int = 0):
+        tau = float(tau)
+        if not (np.isfinite(tau) and tau > 0.0):
+            raise ValueError(f"tau must be finite and > 0 (tau={tau})")
+        self.tau, self.n_rays = tau, _check_rays(n_rays)
+        self.mesh = MeshOccupancy(v, f)
+        self.xyz, self.normal, _ = sample_surface(v, f, n_surface, seed)
+        self._last = None
+
+    def _distance_and_inside(self, queries):
+        last = self._last
+        if last is not None and last[0] is queries and last[1] == queries._version:
+            return last[2]
+        out = self.mesh.distance_and_inside(queries, self.n_rays)
+        self._last = (queries, queries._version, out) if isinstance(queries, torch.Tensor) else None
+        return out
+
+    def torch_attr(self):
+        """(surface samples, their unit normals, None): a mesh has no volume"""
+        return self.xyz, self.normal, None
+
+    def query_sdf(self, queries: torch.Tensor) -> torch.Tensor:
+        """-signed_distance: the distance to the mesh, positive inside and negative on the side the normals of a
+        consistently wound closed mesh point to (PointTSDFVolume.query_sdf's convention)"""
+        dist, inside = self._distance_and_inside(queries)
+        return torch.where(inside, dist, -dist)
+
+    def query_classification(self, queries: torch.Tensor, band: float = 1.0) -> torch.Tensor:
+        """int64 class per query: 1 (empty space) where the query is outside and its distance is >= band * tau (an fp32
+        comparison), 0 everywhere else -- inside a closed mesh the truncated SDF is known, so the near-surface term
+        applies there too.  2 (unknown) is never returned."""
+        dist, inside = self._distance_and_inside(queries)
+        return (~inside & (dist >= band * self.tau)).long()
+
+    def __repr__(self):
+        return f"MeshGroundTruth(triangles={self.mesh.n_tri}, samples={self.xyz.shape[0]}, tau={self.tau})"

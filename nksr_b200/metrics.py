@@ -10,7 +10,8 @@ means and threshold fractions are fp64 reductions in torch.  DESIGN.md SPEC S18 
 
 `o3d-iou` (opt-in, MeshEvaluator(occupancy_rays=K)) is the volumetric IoU of the reference's ONet occupancy samples
 against MeshOccupancy, a ray-parity occupancy of the mesh on an LBVH (csrc/raycast.cu; SPEC S20).  The reference takes
-its occupancy from a package outside its tree, so the value is this project's rule, not a reproduction.
+its occupancy from a package outside its tree, so the value is this project's rule, not a reproduction.  The same BVH
+answers the closest-triangle query (`MeshOccupancy.closest`, `signed_distance`; SPEC S21).
 """
 from __future__ import annotations
 
@@ -134,7 +135,8 @@ class MeshOccupancy:
     """Inside / outside of a triangle mesh by ray parity (SPEC S20): a query is inside when more than half of its K
     rays cross the mesh an odd number of times.  Winding never enters, so triangle soups and mixed orientations are
     fine; on a closed mesh every ray agrees, on an open one the vote is a definition.  The BVH is built once here;
-    `contains` answers any number of query batches.  CUDA only."""
+    `contains` answers any number of query batches, and `closest` / `signed_distance` the distance to the mesh on the
+    same BVH (SPEC S21).  CUDA only."""
 
     def __init__(self, v: torch.Tensor, f: torch.Tensor):
         require_cuda(v, "v")
@@ -171,18 +173,66 @@ class MeshOccupancy:
         """bool (m,): inside by the vote of the first n_rays built-in directions (odd, 1 <= n_rays <= 9)"""
         return occupancy_along(self, points, None, _check_rays(n_rays))
 
+    def closest(self, points):
+        """the closest point of the mesh to every query (SPEC S21): (distance (m,) fp32, closest point (m, 3) fp32,
+        original triangle index (m,) int64).  Equal squared distances go to the lower triangle index; a mesh without
+        triangles gives distance inf, point NaN and index -1.  Bitwise the brute force over every triangle."""
+        dist, point, tri = _closest(self, _queries(self, points))
+        return dist, point, tri.long()
+
+    def signed_distance(self, points, n_rays: int = 3) -> torch.Tensor:
+        """fp32 (m,): the distance of `closest`, negated where `contains(points, n_rays)` is true -- negative inside, as
+        open3d's convention.  The sign is ray parity, not winding."""
+        dist, inside = self.distance_and_inside(points, n_rays)
+        return torch.where(inside, -dist, dist)
+
+    def distance_and_inside(self, points, n_rays: int = 3):
+        """(the distance of `closest`, the bool of `contains(points, n_rays)`) from one validation of the queries"""
+        k = _check_rays(n_rays)
+        q = _queries(self, points)
+        return _closest(self, q)[0], _occupancy(self, q, None, k)
+
     def __repr__(self):
         return f"MeshOccupancy(triangles={self.n_tri}, device={self.device})"
 
 
-def occupancy_along(occ: MeshOccupancy, points, directions=None, n_rays: Optional[int] = None) -> torch.Tensor:
-    """MeshOccupancy.contains with explicit ray directions ((K, 3), K odd in [1, 9], every component nonzero and
-    finite) or, with directions None, the first n_rays built-in ones"""
+def _queries(occ: MeshOccupancy, points) -> torch.Tensor:
+    """the query points as a contiguous fp32 (m, 3) tensor on the mesh's device: CUDA tensors or host arrays,
+    finite"""
     if isinstance(points, torch.Tensor):
         require_cuda(points, "points")
     q = _as_tensor(points, occ.device, torch.float32).reshape(-1, 3)
     if not bool(torch.isfinite(q).all()):
         raise NksrError("query points must be finite")
+    return q
+
+
+def _closest(occ: MeshOccupancy, q: torch.Tensor):
+    """nksr_mesh_closest on checked queries (_queries): distance, point, int32 triangle"""
+    m = q.shape[0]
+    dist = torch.empty(m, dtype=torch.float32, device=occ.device)
+    point = torch.empty((m, 3), dtype=torch.float32, device=occ.device)
+    tri = torch.empty(m, dtype=torch.int32, device=occ.device)
+    if m:
+        call("nksr_mesh_closest", occ.nodes if occ.n_tri > 1 else None, occ.tris if occ.n_tri else None, occ.scene,
+             occ.n_tri, q, m, dist, point, tri, stream_ptr(occ.device))
+    return dist, point, tri
+
+
+def _occupancy(occ: MeshOccupancy, q: torch.Tensor, dirs: Optional[torch.Tensor], k: int) -> torch.Tensor:
+    """nksr_mesh_occupancy on checked queries and ray settings"""
+    m = q.shape[0]
+    inside = torch.empty(m, dtype=torch.uint8, device=occ.device)
+    if m:
+        call("nksr_mesh_occupancy", occ.nodes if occ.n_tri > 1 else None, occ.tris, occ.scene, occ.n_tri, q, m, dirs,
+             k, inside, stream_ptr(occ.device))
+    return inside.bool()
+
+
+def occupancy_along(occ: MeshOccupancy, points, directions=None, n_rays: Optional[int] = None) -> torch.Tensor:
+    """MeshOccupancy.contains with explicit ray directions ((K, 3), K odd in [1, 9], every component nonzero and
+    finite) or, with directions None, the first n_rays built-in ones"""
+    q = _queries(occ, points)
     dirs = None
     if directions is not None:
         dirs = _as_tensor(directions, occ.device, torch.float32).reshape(-1, 3)
@@ -191,12 +241,7 @@ def occupancy_along(occ: MeshOccupancy, points, directions=None, n_rays: Optiona
             raise ValueError("every ray direction component must be finite and nonzero")
     else:
         k = _check_rays(n_rays)
-    m = q.shape[0]
-    inside = torch.empty(m, dtype=torch.uint8, device=occ.device)
-    if m:
-        call("nksr_mesh_occupancy", occ.nodes if occ.n_tri > 1 else None, occ.tris, occ.scene, occ.n_tri, q, m, dirs,
-             k, inside, stream_ptr(occ.device))
-    return inside.bool()
+    return _occupancy(occ, q, dirs, k)
 
 
 def occupancy_iou(pred: torch.Tensor, gt: torch.Tensor) -> float:

@@ -103,8 +103,8 @@ def udf_samples(svh, ref_xyz, ref_normal, voxel_size, samplers=UDF_SAMPLERS, gen
 
 
 def udf_gt(q, ref_xyz, ref_normal, voxel_size, gt_band=GT_BAND, gt=None):
-    """|transform(-sdf_from_points(q, ref, 8, 0.02))|, or with volume ground truth (a PointTSDFVolume)
-    |transform(gt.query_sdf(q))| (models/loss.py:84-86, 111-118)"""
+    """|transform(-sdf_from_points(q, ref, 8, 0.02))|, or with ground truth geometry (a PointTSDFVolume or a
+    MeshGroundTruth) |transform(gt.query_sdf(q))| (models/loss.py:84-86, 111-118)"""
     if gt is not None:
         return transform_field(gt.query_sdf(q), voxel_size, gt_band).abs()
     sdf = -sdf_from_points(q, ref_xyz, ref_normal, 8, 0.02, False)[0]
@@ -115,7 +115,7 @@ def udf_loss(udf_decoder, udf_features, svh: SparseFeatureHierarchy, ref_xyz, re
              samplers=UDF_SAMPLERS, gt_band=GT_BAND, generator=None, q=None, gt=None):
     """mean |transform(pd) - gt| / voxel_size over the UDF samples (models/loss.py:120-140).  pd is the UDF NeuralField
     evaluated differentiably as udf_decoder(NeuralField._interp(q)) on the finest level's UDF features (the decoder
-    takes kernel_dim inputs); `q` overrides the samplers; `gt` (a PointTSDFVolume) gives the ground truth (udf_gt).
+    takes kernel_dim inputs); `q` overrides the samplers; `gt` (ground truth geometry) gives the ground truth (udf_gt).
     Zero when the finest level is empty (a hierarchy grown from a prediction that kept nothing there): there is no
     field to evaluate."""
     if svh.num_voxels(0) == 0:
@@ -144,10 +144,12 @@ def udf_field_loss(udf_decoder, udf_features, svh: SparseFeatureHierarchy, ref_x
 class TrainingScene:
     """one oriented cloud with its encoder hierarchy (point splatting) and ground-truth hierarchy (adaptive, from the
     normals, models/nksr_net.py:175-179).  The decoder runs on the encoder hierarchy: the predicted-structure regime,
-    where all three structure classes occur.  `gt`: volume ground truth (a gt_geometry.PointTSDFVolume on the same
-    device); every loss then takes its reference from it, as models/nksr_net.py and models/loss.py do with
-    DS.GT_GEOMETRY: the ground-truth hierarchy and the surface samples from gt.xyz / gt.normal, the SDF from
-    gt.query_sdf and the spatial loss's empty-space term from gt.query_classification."""
+    where all three structure classes occur.  `gt`: ground truth geometry on the same device, any object with
+    torch_attr() -> (xyz, normal, ...), query_sdf(q) and query_classification(q) (0 near, 1 empty, 2 unknown):
+    gt_geometry.PointTSDFVolume (volume ground truth) or gt_geometry.MeshGroundTruth (a mesh).  Every loss then takes
+    its reference from it, as models/nksr_net.py and models/loss.py do with DS.GT_GEOMETRY: the ground-truth hierarchy and
+    the surface samples from torch_attr(), the SDF from gt.query_sdf and the spatial loss's empty-space term from
+    gt.query_classification."""
 
     def __init__(self, xyz, normal, voxel_size, depth, adaptive_depth=2, gt=None):
         dev = xyz.device
@@ -196,7 +198,8 @@ def spatial_loss(field, ref_xyz, ref_normal, voxel_size, samplers=SPATIAL_SAMPLE
                  gt=None):
     """near-surface L1 of the transformed field against the transformed point-cloud SDF, / voxel_size, over the uniform +
     band samples (models/loss.py:201-260).  Without GT geometry every sample counts as near-surface; with `gt` (a
-    PointTSDFVolume) the loss is spatial_volume_terms' near + empty sums over the number of samples."""
+    PointTSDFVolume or a MeshGroundTruth, see TrainingScene) the loss is spatial_volume_terms' near + empty sums over
+    the number of samples."""
     if gt is not None:
         near, empty, n = spatial_volume_terms(field, ref_xyz, ref_normal, voxel_size, gt, samplers, gt_band, generator)
         return (near + empty) / n
@@ -211,7 +214,7 @@ EMPTY_SPACE_WEIGHT = 0.1     # models/loss.py:244-245: 0.1 exp(pd / (2 voxel_siz
 
 def spatial_volume_terms(field, ref_xyz, ref_normal, voxel_size, gt, samplers=SPATIAL_SAMPLERS, gt_band=GT_BAND,
                          generator=None):
-    """the spatial loss's two sums with volume ground truth (models/loss.py:227-248) and the number of samples:
+    """the spatial loss's two sums with ground truth geometry (models/loss.py:227-248) and the number of samples:
     near = sum over the near-surface samples (class 0 of gt.query_classification) of |transform(pd) -
     transform(gt.query_sdf(q))| / voxel_size; empty = sum over the empty-space samples (class 1) of
     0.1 exp(pd / (2 voxel_size)) of the raw prediction, which pushes the field down in observed free space.  Unknown
@@ -237,7 +240,7 @@ def neural_field(net, feat, dec_svh: SparseFeatureHierarchy):
 def kernel_losses(net, scene: TrainingScene, generator=None, feat=None, dec_svh=None, timer=None, operator=None):
     """the field losses of a trainable NKSRNetwork on the scene: dict(total, gt_value, gt_normal, spatial, field), on
     the KernelField (kernel_field), or with geometry='neural' on the NeuralField (neural_field, no solve).  `feat`,
-    `dec_svh`: an existing forward of the network (else one is run).  With volume ground truth (scene.gt) the dict
+    `dec_svh`: an existing forward of the network (else one is run).  With ground truth geometry (scene.gt) the dict
     also holds spatial_empty, the empty-space term's share of spatial.  `operator`: the kernel solve's (kernel_field)."""
     if feat is None:
         enc = net.encoder(scene.xyz, scene.normal, scene.enc_svh, 0)

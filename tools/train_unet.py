@@ -32,6 +32,8 @@ the crop's sensor rays (csrc/tsdf_volume.cu, DESIGN.md SPEC S19) with node spaci
 margin of one top-level voxel around the points -- our choices, the reference ships its volumes as data.  The setup
 line reports the build time and the near / free / unknown fractions of the nodes; with --kernel-losses every step
 reports the spatial loss's empty-space term (spatial_empty).
+--mesh-gt (sphere only) trains against a mesh: MeshGroundTruth (DESIGN.md SPEC S21) of a level-6 icosphere (81,920
+triangles) of the scene's radius 0.35, tau = 2 W, its SDF the exact distance to the triangles signed by ray parity.
 --out saves {'state_dict': ...}, which load_checkpoint_from_url(<path>) + load_state_dict take."""
 import argparse
 import json
@@ -66,8 +68,21 @@ def build_volume(px, pn, ps, W, depth):
     return PointTSDFVolume.from_sensor_rays(px, pn, ps, h=W, tau=2.0 * W, margin=W * 2 ** (depth - 1))
 
 
-def make_scene(kind, n, depth, device, vol_sup=False):
-    """the TrainingScene, and with vol_sup the volume's grid, build time (ms) and class fractions"""
+MESH_GT_LEVEL = 6       # --mesh-gt: 81,920 triangles, the size of a ShapeNet model
+
+
+def build_mesh_gt(W, device):
+    """the mesh ground truth of --mesh-gt: an icosphere of radius 0.35 (tests.clouds.sphere's), tau = 2 W"""
+    import torch
+    from nksr_b200.gt_geometry import MeshGroundTruth
+    from tests.test_cpu_occupancy import icosphere
+    v, f = icosphere(MESH_GT_LEVEL, 0.35)
+    return MeshGroundTruth(torch.from_numpy(v).to(device), torch.from_numpy(f).to(device), tau=2.0 * W)
+
+
+def make_scene(kind, n, depth, device, vol_sup=False, mesh_gt=False):
+    """the TrainingScene, and with vol_sup the volume's grid, build time (ms) and class fractions; with mesh_gt the
+    mesh's triangles and set-up time (ms, the icosphere's construction on the host included)"""
     import numpy as np
     import torch
     from nksr_b200.training import TrainingScene
@@ -75,7 +90,17 @@ def make_scene(kind, n, depth, device, vol_sup=False):
     if kind == "sphere":
         from tests import clouds
         xyz, nrm = clouds.sphere(n, noise=0.001)
-        return TrainingScene(t(xyz), t(nrm), 0.02 if n <= 300_000 else 0.01, depth), None
+        W = 0.02 if n <= 300_000 else 0.01
+        if not mesh_gt:
+            return TrainingScene(t(xyz), t(nrm), W, depth), None
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        gt = build_mesh_gt(W, device)
+        e1.record()
+        torch.cuda.synchronize()
+        return (TrainingScene(t(xyz), t(nrm), W, depth, gt=gt),
+                dict(triangles=gt.mesh.n_tri, samples=int(gt.xyz.shape[0]), tau=gt.tau,
+                     setup_ms=round(e0.elapsed_time(e1), 3)))
     px, pn, ps, W = cfg4_crop(n, device)
     if not vol_sup:
         return TrainingScene(px, pn, W, depth), None
@@ -204,6 +229,8 @@ def main(argv=None):
                     help="udf.enabled: the UDF loss on the NeuralField over every level (DESIGN.md SPEC S17)")
     ap.add_argument("--vol-sup", action="store_true",
                     help="cfg4: volume ground truth from the sensor rays (DESIGN.md SPEC S19)")
+    ap.add_argument("--mesh-gt", action="store_true",
+                    help="sphere: mesh ground truth, an icosphere of the scene's radius (DESIGN.md SPEC S21)")
     ap.add_argument("--operator", choices=("assembled", "matrix_free"), default=None,
                     help="--kernel-losses: the kernel solve's operator (default: assembled)")
     ap.add_argument("--geometry", choices=("kernel", "neural"), default="kernel",
@@ -215,6 +242,8 @@ def main(argv=None):
         ap.error("--steps must be >= 1")
     if args.vol_sup and args.scene != "cfg4":
         ap.error("--vol-sup needs --scene cfg4 (its points carry their sensor positions)")
+    if args.mesh_gt and args.scene != "sphere":
+        ap.error("--mesh-gt needs --scene sphere (its ground-truth mesh is the icosphere of the same radius)")
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("train_unet.py needs a CUDA device")
@@ -225,7 +254,7 @@ def main(argv=None):
     from nksr_b200.network import NKSRNetwork
     torch.use_deterministic_algorithms(True, warn_only=True)
     dev = torch.device("cuda:0")
-    scene, vol = make_scene(args.scene, args.points, args.depth, dev, args.vol_sup)
+    scene, vol = make_scene(args.scene, args.points, args.depth, dev, args.vol_sup, args.mesh_gt)
     net = NKSRNetwork(dict(backbone="unet", tree_depth=args.depth, kernel_dim=4, precision=args.precision,
                            trainable=True, seed=args.seed, structure=args.structure,
                            udf=dict(enabled=args.udf), geometry=args.geometry)).to(dev)
@@ -237,7 +266,7 @@ def main(argv=None):
                 pd_structure_prob=args.pd_structure_prob, udf=args.udf, geometry=args.geometry, operator=args.operator,
                 voxels=[scene.enc_svh.num_voxels(l) for l in range(args.depth)])
     if vol is not None:
-        info["volume"] = vol
+        info["mesh_gt" if args.mesh_gt else "volume"] = vol
     print(json.dumps(dict(setup=info)), flush=True)
     rows = []
     for step in range(args.steps):
