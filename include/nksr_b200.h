@@ -567,7 +567,15 @@ NKSR_API int nksr_tsdf_volume(const float* xyz, const float* sensor, int64_t n, 
  * nksr_mesh_closest (SPEC S21): for every query[i] (float[m*3], finite) the closest triangle of the mesh on the same
  * BVH: dist[i] (float[m]) = sqrt(d2), point[i] (float[m*3]) = the closest point whose d2 that is, tri[i] (int32[m]) =
  * the original triangle index; equal d2 go to the lower index.  Equal bit for bit to testing every triangle (the box
- * bound is conservative); n_tri = 0 gives dist inf, point NaN, tri -1. */
+ * bound is conservative); n_tri = 0 gives dist inf, point NaN, tri -1.
+ * nksr_mesh_first_hit (SPEC S22): for every ray i from origin[i] along dir[i] (float[m*3] each, finite, dir not all
+ * zero, zero components allowed) the first triangle the ray crosses by S20's test at 0 < t <= t_max[i] (float[m],
+ * not NaN; t_max NULL: t_max_all for every ray), t = T / det in fp64; equal t go to the lower original index.
+ * t[i] (float[m]) = that t rounded to fp32, point[i] (float[m*3]) = origin + t[i] * dir, normal[i] (float[m*3]) =
+ * (v1 - v0) x (v2 - v0) / |.| of the original triangle f (int32[n_tri*3]) over v (float[V*3]), the mesh the BVH was
+ * built from (NaN for a zero cross product), tri[i] (int32[m]) = the original triangle index.  A miss, and n_tri = 0,
+ * give t inf, point and normal NaN, tri -1.  Equal bit for bit to testing every triangle (the slab entry is a
+ * conservative bound on t).  Caller-owned buffers, no allocation. */
 NKSR_API size_t nksr_bvh_workspace_bytes(int64_t n_tri);
 NKSR_API int nksr_bvh_keys(const float* v, const int32_t* f, int64_t n_tri, float* scene, int64_t* keys, int32_t* idx,
                            void* stream);
@@ -580,6 +588,10 @@ NKSR_API int nksr_mesh_occupancy(const float* nodes, const float* tris, const fl
                                  void* stream);
 NKSR_API int nksr_mesh_closest(const float* nodes, const float* tris, const float* scene, int64_t n_tri,
                                const float* query, int64_t m, float* dist, float* point, int32_t* tri, void* stream);
+NKSR_API int nksr_mesh_first_hit(const float* nodes, const float* tris, const float* scene, int64_t n_tri,
+                                 const float* v, const int32_t* f, const float* origin, const float* dir, int64_t m,
+                                 const float* t_max, float t_max_all, float* t, float* point, float* normal,
+                                 int32_t* tri, void* stream);
 
 #ifdef __cplusplus
 }

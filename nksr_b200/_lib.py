@@ -154,6 +154,7 @@ _SIGNATURES = {
     "nksr_bvh_refit": ("i", "pppqpppzp"),
     "nksr_mesh_occupancy": ("i", "pppqpqpipp"),
     "nksr_mesh_closest": ("i", "pppqpqpppp"),
+    "nksr_mesh_first_hit": ("i", "pppqpppp" + "qpf" + "ppppp"),
 }
 
 _lib = None

@@ -19,6 +19,11 @@
 // exceeds the routine's d2 of any triangle inside, so the answer, ties to the lower original index included, is the
 // brute force's bit for bit.
 //
+// First hit: k_mesh_first_hit, one thread per ray (its own origin, direction and t_max), nearest-entry-first over the
+// same LBVH.  SPEC S22's candidates are S20's crossings, each at t = T / det; a child box is skipped only when its
+// padded slab entry is strictly above the best t so far or t_max, and that entry never exceeds the t of a candidate
+// inside, so the hit, ties to the lower original index included, is the brute force's bit for bit.
+//
 // Built with --fmad=false: the rules round every fp32 and fp64 product and sum on their own (SPEC S20, S21).
 #include "common.cuh"
 
@@ -251,15 +256,22 @@ k_bvh_refit(const float* __restrict__ v, const int32_t* __restrict__ f, const in
 }
 
 // Ize's slab test on the box padded by pad: origin o, reciprocal direction r; the far distance is inflated by
-// 1 + 2^-20 (> 1 + 2 gamma_3), and only t >= 0 counts
-__device__ __forceinline__ bool slab_hit(const float4 lo, const float4 hi, const float pad, const float o[3],
-                                         const float r[3]) {
+// 1 + 2^-20 (> 1 + 2 gamma_3), and only t >= 0 counts.  tn is the entry distance (in units of the direction), which
+// the first-hit traversal orders and bounds by (DESIGN.md section 4.7)
+__device__ __forceinline__ bool slab_entry(const float4 lo, const float4 hi, const float pad, const float o[3],
+                                           const float r[3], float& tn) {
   const float t0x = (lo.x - pad - o[0]) * r[0], t1x = (hi.x + pad - o[0]) * r[0];
   const float t0y = (lo.y - pad - o[1]) * r[1], t1y = (hi.y + pad - o[1]) * r[1];
   const float t0z = (lo.z - pad - o[2]) * r[2], t1z = (hi.z + pad - o[2]) * r[2];
-  const float tn = fmaxf(fmaxf(fminf(t0x, t1x), fminf(t0y, t1y)), fminf(t0z, t1z));
+  tn = fmaxf(fmaxf(fminf(t0x, t1x), fminf(t0y, t1y)), fminf(t0z, t1z));
   const float tf = fminf(fminf(fmaxf(t0x, t1x), fmaxf(t0y, t1y)), fmaxf(t0z, t1z)) * (1.f + 0x1p-20f);
   return tf >= 0.f && tn <= tf;
+}
+
+__device__ __forceinline__ bool slab_hit(const float4 lo, const float4 hi, const float pad, const float o[3],
+                                         const float r[3]) {
+  float tn;
+  return slab_entry(lo, hi, pad, o, r, tn);
 }
 
 // the ray's frame (SPEC S20): kz = argmax |d| (first on ties), kx, ky the next two cyclically, swapped when d[kz] < 0
@@ -267,6 +279,19 @@ struct RayFrame {
   int kx, ky, kz;
   float sx, sy, sz;
 };
+
+__device__ __forceinline__ RayFrame ray_frame(const float d[3]) {
+  int kz = 0;
+  if (fabsf(d[1]) > fabsf(d[kz])) kz = 1;
+  if (fabsf(d[2]) > fabsf(d[kz])) kz = 2;
+  int kx = kz == 2 ? 0 : kz + 1, ky = kx == 2 ? 0 : kx + 1;
+  if (d[kz] < 0.f) {
+    const int s = kx;
+    kx = ky;
+    ky = s;
+  }
+  return {kx, ky, kz, __fdiv_rn(d[kx], d[kz]), __fdiv_rn(d[ky], d[kz]), __fdiv_rn(1.f, d[kz])};
+}
 
 __device__ __forceinline__ float pick(const float a[3], int k) { return k == 0 ? a[0] : (k == 1 ? a[1] : a[2]); }
 
@@ -276,9 +301,10 @@ __device__ __forceinline__ bool owns(const float px, const float py, const float
   return pos ? (qy > py || (qy == py && px > qx)) : (qy < py || (qy == py && px < qx));
 }
 
-// SPEC S20's crossing test of the ray from the query (o) along the frame's direction with triangle t
-__device__ __forceinline__ bool crosses(const float4* __restrict__ tris, const int64_t t, const float o[3],
-                                        const RayFrame& fr) {
+// SPEC S20's crossing test of the ray from the query (o) along the frame's direction with triangle t; on a crossing
+// the ray parameter of SPEC S22 is T / det
+__device__ __forceinline__ bool crossing(const float4* __restrict__ tris, const int64_t t, const float o[3],
+                                         const RayFrame& fr, double& T, double& det) {
   float sx[3], sy[3], sz[3];
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
@@ -293,14 +319,20 @@ __device__ __forceinline__ bool crosses(const float4* __restrict__ tris, const i
   double V = (double)sx[0] * sy[2] - (double)sy[0] * sx[2];
   double W = (double)sx[1] * sy[0] - (double)sy[1] * sx[0];
   if ((U < 0.0 || V < 0.0 || W < 0.0) && (U > 0.0 || V > 0.0 || W > 0.0)) return false;
-  const double det = U + V + W;
+  det = U + V + W;
   if (det == 0.0) return false;
   const bool pos = det > 0.0;
   if (U == 0.0 && !owns(sx[1], sy[1], sx[2], sy[2], pos)) return false;
   if (V == 0.0 && !owns(sx[2], sy[2], sx[0], sy[0], pos)) return false;
   if (W == 0.0 && !owns(sx[0], sy[0], sx[1], sy[1], pos)) return false;
-  const double T = U * (double)sz[0] + V * (double)sz[1] + W * (double)sz[2];
+  T = U * (double)sz[0] + V * (double)sz[1] + W * (double)sz[2];
   return pos ? T > 0.0 : T < 0.0;
+}
+
+__device__ __forceinline__ bool crosses(const float4* __restrict__ tris, const int64_t t, const float o[3],
+                                        const RayFrame& fr) {
+  double T, det;
+  return crossing(tris, t, o, fr, T, det);
 }
 
 __global__ void __launch_bounds__(kOccThreads)
@@ -313,16 +345,7 @@ k_mesh_occupancy(const float4* __restrict__ nodes, const float4* __restrict__ tr
     const int r = threadIdx.x;
     const float d[3] = {dirs ? dirs[3 * r] : kDefaultDirs[r][0], dirs ? dirs[3 * r + 1] : kDefaultDirs[r][1],
                         dirs ? dirs[3 * r + 2] : kDefaultDirs[r][2]};
-    int kz = 0;
-    if (fabsf(d[1]) > fabsf(d[kz])) kz = 1;
-    if (fabsf(d[2]) > fabsf(d[kz])) kz = 2;
-    int kx = kz == 2 ? 0 : kz + 1, ky = kx == 2 ? 0 : kx + 1;
-    if (d[kz] < 0.f) {
-      const int s = kx;
-      kx = ky;
-      ky = s;
-    }
-    frames[r] = {kx, ky, kz, __fdiv_rn(d[kx], d[kz]), __fdiv_rn(d[ky], d[kz]), __fdiv_rn(1.f, d[kz])};
+    frames[r] = ray_frame(d);
 #pragma unroll
     for (int k = 0; k < 3; ++k) recip[r][k] = __fdiv_rn(1.f, d[k]);
   }
@@ -547,6 +570,110 @@ k_mesh_closest(const float4* __restrict__ nodes, const float4* __restrict__ tris
   tri[i] = n_tri > 0 ? best.tri : -1;
 }
 
+// ---- SPEC S22: the first hit of a ray, the candidates of SPEC S20 ordered by t = T / det.
+
+constexpr int kHitThreads = 128;
+
+// the leaf-order triangle j against the best hit so far: a crossing with 0 < t <= t_max (fp64) replaces it when its
+// t is smaller, or equal with a lower original index
+__device__ __forceinline__ void test_hit(const float4* __restrict__ tris, const int32_t j, const float o[3],
+                                         const RayFrame& fr, const double t_max, double& best_t, int32_t& best_tri) {
+  double T, det;
+  if (!crossing(tris, j, o, fr, T, det)) return;
+  const double t = __ddiv_rn(T, det);
+  const int32_t id = __float_as_int(__ldg(&tris[3 * (int64_t)j].w));
+  if (t > 0.0 && t <= t_max && (t < best_t || (t == best_t && id < best_tri))) {
+    best_t = t;
+    best_tri = id;
+  }
+}
+
+__global__ void __launch_bounds__(kHitThreads)
+k_mesh_first_hit(const float4* __restrict__ nodes, const float4* __restrict__ tris, const float* __restrict__ scene,
+                 const int64_t n_tri, const float* __restrict__ v, const int32_t* __restrict__ f,
+                 const float* __restrict__ origin, const float* __restrict__ dir, const int64_t m,
+                 const float* __restrict__ t_max, const float t_max_all, float* __restrict__ t_out,
+                 float* __restrict__ point, float* __restrict__ normal, int32_t* __restrict__ tri) {
+  const int64_t i = blockIdx.x * (int64_t)kHitThreads + threadIdx.x;
+  if (i >= m) return;
+  const float o[3] = {__ldg(origin + 3 * i), __ldg(origin + 3 * i + 1), __ldg(origin + 3 * i + 2)};
+  const float d[3] = {__ldg(dir + 3 * i), __ldg(dir + 3 * i + 1), __ldg(dir + 3 * i + 2)};
+  const double tmax = (double)(t_max ? __ldg(t_max + i) : t_max_all);
+  // INT32_MAX: no candidate yet, so a candidate with t = inf (an overflow) still ties in as the brute force's does
+  double best_t = INFINITY;
+  int32_t best_tri = INT32_MAX;
+  if (n_tri > 0) {
+    const RayFrame fr = ray_frame(d);
+    if (n_tri == 1) {
+      test_hit(tris, 0, o, fr, tmax, best_t, best_tri);
+    } else {
+      const float rc[3] = {__fdiv_rn(1.f, d[0]), __fdiv_rn(1.f, d[1]), __fdiv_rn(1.f, d[2])};
+      // S20's padding: the entry distance of the padded box never exceeds the t of a candidate inside (section 4.7)
+      const float pad = (__ldg(scene + 6) + fmaxf(fabsf(o[0]), fmaxf(fabsf(o[1]), fabsf(o[2])))) * 0x1p-19f;
+      int32_t stack[kStack];
+      float stack_tn[kStack];
+      int sp = 0;
+      int32_t node = 0;
+      for (;;) {
+        const float4* nd = nodes + 4 * (int64_t)node;
+        const float4 a = __ldg(nd), b = __ldg(nd + 1), c = __ldg(nd + 2), e = __ldg(nd + 3);
+        float tn0, tn1;
+        const bool h0 = slab_entry(a, b, pad, o, rc, tn0), h1 = slab_entry(c, e, pad, o, rc, tn1);
+        const bool swap = h1 && (!h0 || tn1 < tn0);     // nearer entry first, child 0 on equal entries
+        const int32_t near = __float_as_int(swap ? b.w : a.w), far = __float_as_int(swap ? a.w : b.w);
+        const bool near_h = swap ? h1 : h0, far_h = swap ? h0 : h1;
+        const float near_tn = swap ? tn1 : tn0, far_tn = swap ? tn0 : tn1;
+        // a box is skipped only when its entry is strictly beyond the best t or t_max
+        int32_t next = -1;
+        if (near_h && !((double)near_tn > fmin(best_t, tmax))) {
+          if (near < 0) test_hit(tris, ~near, o, fr, tmax, best_t, best_tri);
+          else next = near;
+        }
+        if (far_h && !((double)far_tn > fmin(best_t, tmax))) {
+          if (far < 0) {
+            test_hit(tris, ~far, o, fr, tmax, best_t, best_tri);
+          } else if (next < 0) {
+            next = far;
+          } else {
+            stack[sp] = far;
+            stack_tn[sp++] = far_tn;
+          }
+        }
+        while (next < 0 && sp > 0) {
+          --sp;
+          if (!((double)stack_tn[sp] > fmin(best_t, tmax))) next = stack[sp];
+        }
+        if (next < 0) break;
+        node = next;
+      }
+    }
+  }
+  const bool hit = best_tri != INT32_MAX;
+  const float t32 = hit ? __double2float_rn(best_t) : INFINITY;
+  float n[3] = {NAN, NAN, NAN};
+  if (hit) {
+    // the normal in the caller's winding: (v1 - v0) x (v2 - v0), normalised
+    float p[3][3], e1[3], e2[3];
+    load_tri(v, f, best_tri, p);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      e1[k] = p[1][k] - p[0][k];
+      e2[k] = p[2][k] - p[0][k];
+    }
+    cross3(e1, e2, n);
+    const float len = __fsqrt_rn(dot3(n, n));
+#pragma unroll
+    for (int k = 0; k < 3; ++k) n[k] = __fdiv_rn(n[k], len);
+  }
+  t_out[i] = t32;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    point[3 * i + k] = hit ? __fadd_rn(o[k], __fmul_rn(t32, d[k])) : NAN;
+    normal[3 * i + k] = n[k];
+  }
+  tri[i] = hit ? best_tri : -1;
+}
+
 }  // namespace
 
 extern "C" {
@@ -628,6 +755,20 @@ int nksr_mesh_closest(const float* nodes, const float* tris, const float* scene,
   k_mesh_closest<<<grid_for(m, kDistThreads), kDistThreads, 0, as_stream(stream)>>>(
       reinterpret_cast<const float4*>(nodes), reinterpret_cast<const float4*>(tris), scene, n_tri, query, m, dist,
       point, tri);
+  NKSR_CHECK_LAUNCH();
+  return NKSR_OK;
+}
+
+int nksr_mesh_first_hit(const float* nodes, const float* tris, const float* scene, int64_t n_tri, const float* v,
+                        const int32_t* f, const float* origin, const float* dir, int64_t m, const float* t_max,
+                        float t_max_all, float* t, float* point, float* normal, int32_t* tri, void* stream) {
+  if (n_tri < 0 || n_tri > INT32_MAX || m < 0) return NKSR_E_INVALID;
+  if (m == 0) return NKSR_OK;
+  if (!origin || !dir || !t || !point || !normal || !tri) return NKSR_E_INVALID;
+  if (n_tri > 0 && (!tris || !scene || !v || !f || (n_tri > 1 && !nodes))) return NKSR_E_INVALID;
+  k_mesh_first_hit<<<grid_for(m, kHitThreads), kHitThreads, 0, as_stream(stream)>>>(
+      reinterpret_cast<const float4*>(nodes), reinterpret_cast<const float4*>(tris), scene, n_tri, v, f, origin, dir,
+      m, t_max, t_max_all, t, point, normal, tri);
   NKSR_CHECK_LAUNCH();
   return NKSR_OK;
 }

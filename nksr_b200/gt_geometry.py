@@ -15,10 +15,18 @@ Mesh ground truth for object datasets (a closed mesh such as ShapeNet's), SPEC S
     gt = MeshGroundTruth(v, f, tau)                       # the BVH of metrics.MeshOccupancy, surface samples
     sdf = gt.query_sdf(q)                                 # -signed_distance: positive inside
     cls = gt.query_classification(q)                      # 1 outside with |sdf| >= band tau, else 0
+
+Simulated LiDAR scans of a mesh, for sensor-bearing input with exact ground truth (SPEC S22, the first hit on the
+same BVH):
+
+    dirs = lidar_directions(64, 1024)                     # a spinning scanner's unit directions, our pattern
+    xyz, sensor, normal, tri = scan_mesh(gt.mesh, sensors, dirs, max_range=...)
 """
 from __future__ import annotations
 
 import ctypes as C
+import math
+from typing import NamedTuple
 
 import numpy as np
 import torch
@@ -194,3 +202,74 @@ class MeshGroundTruth:
 
     def __repr__(self):
         return f"MeshGroundTruth(triangles={self.mesh.n_tri}, samples={self.xyz.shape[0]}, tau={self.tau})"
+
+
+def lidar_directions(n_beams: int = 64, n_azimuth: int = 1024, elevation_deg=(-24.8, 2.0)) -> torch.Tensor:
+    """unit fp32 directions of a spinning scanner, (n_beams * n_azimuth, 3) on the host: azimuth step k (the outer
+    index) at 2 pi (k + 1/2) / n_azimuth from +x towards +y, beam j (the inner index) at the elevation
+    lo + (hi - lo) j / (n_beams - 1) above the xy plane (lo alone for one beam), each direction
+    (cos e cos a, cos e sin a, sin e) formed in fp64 and rounded once.  The default is a 64-beam sensor's vertical field
+    of view; the pattern is this project's definition, not any vendor's firing order."""
+    n_beams, n_azimuth = int(n_beams), int(n_azimuth)
+    if n_beams < 1 or n_azimuth < 1:
+        raise ValueError(f"n_beams and n_azimuth must be >= 1 (got {n_beams}, {n_azimuth})")
+    lo, hi = (float(x) for x in elevation_deg)
+    if not (np.isfinite(lo) and np.isfinite(hi) and -90.0 <= lo <= hi <= 90.0):
+        raise ValueError(f"elevation_deg must be finite with -90 <= lo <= hi <= 90 (got {elevation_deg})")
+    e = np.deg2rad(lo + (hi - lo) * np.arange(n_beams) / max(n_beams - 1, 1))
+    a = 2.0 * np.pi * (np.arange(n_azimuth) + 0.5) / n_azimuth
+    ce = np.cos(e)[None, :]
+    d = np.stack([ce * np.cos(a)[:, None], ce * np.sin(a)[:, None],
+                  np.broadcast_to(np.sin(e)[None, :], (n_azimuth, n_beams))], axis=-1)
+    return torch.from_numpy(np.ascontiguousarray(d.reshape(-1, 3).astype(np.float32)))
+
+
+class MeshScan(NamedTuple):
+    """the returns of scan_mesh, in ray order: point, the sensor position it was seen from, the unit normal of the hit
+    triangle (its winding) and the original triangle index (int64)"""
+    xyz: torch.Tensor
+    sensor: torch.Tensor
+    normal: torch.Tensor
+    tri: torch.Tensor
+
+
+SCAN_BATCH = 1 << 22      # rays per intersect call in scan_mesh: about 200 MB of ray and hit buffers
+
+
+def scan_mesh(mesh: MeshOccupancy, sensors, directions, max_range: float = math.inf, range_noise: float = 0.0,
+              generator=None) -> MeshScan:
+    """a simulated scan of the mesh: every direction ((R, 3), e.g. lidar_directions()) cast from every sensor position
+    ((P, 3)), ray p R + r from sensors[p] along directions[r] (pose-major), in batches of SCAN_BATCH rays.  The returns
+    are the first hits (MeshOccupancy.intersect, SPEC S22) with t <= max_range -- t is in units of the direction, so
+    with unit directions it is the range -- kept in ray order.  With range_noise > 0 each point moves along its unit
+    ray by range_noise times a standard normal drawn from `generator` (one draw per return, in order); with 0 nothing
+    is drawn and the scan is bitwise reproducible.  Sensors and directions may be host arrays or tensors."""
+    dev = mesh.device
+    max_range, range_noise = float(max_range), float(range_noise)
+    if math.isnan(max_range):
+        raise ValueError("max_range must not be NaN")
+    if not (math.isfinite(range_noise) and range_noise >= 0.0):
+        raise ValueError(f"range_noise must be finite and >= 0 (got {range_noise})")
+    s = torch.as_tensor(sensors).detach().to(dev, torch.float32).reshape(-1, 3).contiguous()
+    d = torch.as_tensor(directions).detach().to(dev, torch.float32).reshape(-1, 3).contiguous()
+    P, R = s.shape[0], d.shape[0]
+    parts = []
+    for start in range(0, P * R, SCAN_BATCH):
+        ray = torch.arange(start, min(start + SCAN_BATCH, P * R), device=dev)
+        o, dr = s[ray // R], d[ray % R]
+        t, point, normal, tri = mesh.intersect(o, dr, max_range)
+        keep = (tri >= 0).to(torch.int32)
+        scan = _lib.exclusive_scan32(keep)
+        cnt = int(scan[-1].item())
+        rows = [point, o, normal, tri] + ([dr] if range_noise > 0.0 else [])
+        parts.append([_lib.compact_rows(a.contiguous(), keep, scan, cnt) for a in rows])
+    if not parts:
+        e3 = torch.empty((0, 3), dtype=torch.float32, device=dev)
+        return MeshScan(e3, e3.clone(), e3.clone(), torch.empty(0, dtype=torch.int64, device=dev))
+    cols = [torch.cat(c) for c in zip(*parts)]
+    xyz, sensor, normal, tri = cols[:4]
+    if range_noise > 0.0:
+        u = cols[4] / torch.linalg.vector_norm(cols[4], dim=1, keepdim=True)
+        eps = torch.randn((xyz.shape[0], 1), generator=generator, device=dev, dtype=torch.float32)
+        xyz = xyz + (range_noise * eps) * u
+    return MeshScan(xyz, sensor, normal, tri)

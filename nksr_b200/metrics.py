@@ -11,7 +11,8 @@ means and threshold fractions are fp64 reductions in torch.  DESIGN.md SPEC S18 
 `o3d-iou` (opt-in, MeshEvaluator(occupancy_rays=K)) is the volumetric IoU of the reference's ONet occupancy samples
 against MeshOccupancy, a ray-parity occupancy of the mesh on an LBVH (csrc/raycast.cu; SPEC S20).  The reference takes
 its occupancy from a package outside its tree, so the value is this project's rule, not a reproduction.  The same BVH
-answers the closest-triangle query (`MeshOccupancy.closest`, `signed_distance`; SPEC S21).
+answers the closest-triangle query (`MeshOccupancy.closest`, `signed_distance`; SPEC S21) and the first hit of a ray
+(`MeshOccupancy.intersect`; SPEC S22).
 """
 from __future__ import annotations
 
@@ -135,8 +136,8 @@ class MeshOccupancy:
     """Inside / outside of a triangle mesh by ray parity (SPEC S20): a query is inside when more than half of its K
     rays cross the mesh an odd number of times.  Winding never enters, so triangle soups and mixed orientations are
     fine; on a closed mesh every ray agrees, on an open one the vote is a definition.  The BVH is built once here;
-    `contains` answers any number of query batches, and `closest` / `signed_distance` the distance to the mesh on the
-    same BVH (SPEC S21).  CUDA only."""
+    `contains` answers any number of query batches, `closest` / `signed_distance` the distance to the mesh on the
+    same BVH (SPEC S21) and `intersect` the first hit of a ray (SPEC S22).  CUDA only."""
 
     def __init__(self, v: torch.Tensor, f: torch.Tensor):
         require_cuda(v, "v")
@@ -153,6 +154,8 @@ class MeshOccupancy:
             raise NksrError("mesh vertices must be finite")
         f = f.to(torch.int32).contiguous()
         self.device, self.n_tri = dev, t
+        self.v, self.f = v, f               # the first hit's normal is taken in the caller's winding
+
         self.scene = torch.zeros(8, dtype=torch.float32, device=dev)
         self.nodes = torch.empty((max(t - 1, 0), 16), dtype=torch.float32, device=dev)
         self.tris = torch.empty((t, 12), dtype=torch.float32, device=dev)
@@ -192,6 +195,45 @@ class MeshOccupancy:
         q = _queries(self, points)
         return _closest(self, q)[0], _occupancy(self, q, None, k)
 
+    def intersect(self, origins, directions, t_max=None):
+        """the first hit of every ray from origins[i] along directions[i] (SPEC S22; (m, 3) each, finite, no direction
+        all zero): (t (m,) fp32, point = origin + t * direction (m, 3) fp32, unit normal of the hit triangle in its
+        (v1 - v0) x (v2 - v0) winding (m, 3) fp32, original triangle index (m,) int64).  Only hits at 0 < t <= t_max
+        count (None: +inf; a number, or one value per ray); t is in units of the direction's length.  Equal t go to
+        the lower triangle index.  A miss, and every ray of a mesh without triangles, gives t inf, point and normal
+        NaN and index -1.  Bitwise the brute force over every triangle."""
+        o = _ray_array(self, origins, "origins")
+        d = _ray_array(self, directions, "directions")
+        m = o.shape[0]
+        if d.shape[0] != m:
+            raise ValueError(f"{m} origins but {d.shape[0]} directions")
+        if m and not bool((d != 0).any(dim=1).all()):
+            raise ValueError("every ray direction needs a nonzero component")
+        t_all, t_ray = math.inf, None
+        if t_max is not None:
+            if isinstance(t_max, torch.Tensor) and t_max.dim() > 0 or isinstance(t_max, (np.ndarray, list, tuple)):
+                if isinstance(t_max, torch.Tensor):
+                    require_cuda(t_max, "t_max")
+                t_ray = _as_tensor(t_max, self.device, torch.float32).reshape(-1)
+                if t_ray.shape[0] != m:
+                    raise ValueError(f"t_max has {t_ray.shape[0]} values for {m} rays")
+                if bool(torch.isnan(t_ray).any()):
+                    raise ValueError("t_max must not be NaN")
+            else:
+                t_all = float(np.float32(float(t_max)))
+                if math.isnan(t_all):
+                    raise ValueError("t_max must not be NaN")
+        t = torch.empty(m, dtype=torch.float32, device=self.device)
+        point = torch.empty((m, 3), dtype=torch.float32, device=self.device)
+        normal = torch.empty((m, 3), dtype=torch.float32, device=self.device)
+        tri = torch.empty(m, dtype=torch.int32, device=self.device)
+        if m:
+            has = self.n_tri > 0
+            call("nksr_mesh_first_hit", self.nodes if self.n_tri > 1 else None, self.tris if has else None,
+                 self.scene, self.n_tri, self.v if has else None, self.f if has else None, o, d, m, t_ray, t_all, t,
+                 point, normal, tri, stream_ptr(self.device))
+        return t, point, normal, tri.long()
+
     def __repr__(self):
         return f"MeshOccupancy(triangles={self.n_tri}, device={self.device})"
 
@@ -205,6 +247,16 @@ def _queries(occ: MeshOccupancy, points) -> torch.Tensor:
     if not bool(torch.isfinite(q).all()):
         raise NksrError("query points must be finite")
     return q
+
+
+def _ray_array(occ: MeshOccupancy, a, what: str) -> torch.Tensor:
+    """ray origins or directions as a contiguous fp32 (m, 3) tensor on the mesh's device, checked as _queries does"""
+    if isinstance(a, torch.Tensor):
+        require_cuda(a, what)
+    x = _as_tensor(a, occ.device, torch.float32).reshape(-1, 3)
+    if not bool(torch.isfinite(x).all()):
+        raise NksrError(f"ray {what} must be finite")
+    return x
 
 
 def _closest(occ: MeshOccupancy, q: torch.Tensor):

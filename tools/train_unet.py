@@ -9,6 +9,7 @@ the structure and UDF losses (nksr_b200/training.py), Adam lr 1e-4, gradient nor
     python tools/train_unet.py --scene sphere --points 200000 --depth 4 --geometry neural --steps 30
     python tools/train_unet.py --scene cfg4 --points 1000000 --depth 4 --kernel-losses --vol-sup --steps 10
     python tools/train_unet.py --scene cfg4 --points 1000000 --depth 4 --kernel-losses --operator matrix_free --steps 10
+    python tools/train_unet.py --scene sphere --mesh-gt --mesh-scan --steps 10
 
 Scenes: 'sphere' (tests/clouds.py, exact normals) or 'cfg4' (a crop of bench.py's outdoor scene at its own density,
 normals from the kNN preprocess).  Every step prints one JSON line: the losses and the CUDA-event times of the forward,
@@ -34,6 +35,11 @@ line reports the build time and the near / free / unknown fractions of the nodes
 reports the spatial loss's empty-space term (spatial_empty).
 --mesh-gt (sphere only) trains against a mesh: MeshGroundTruth (DESIGN.md SPEC S21) of a level-6 icosphere (81,920
 triangles) of the scene's radius 0.35, tau = 2 W, its SDF the exact distance to the triangles signed by ray parity.
+--mesh-scan (with --mesh-gt) takes the input from a simulated LiDAR scan of that icosphere instead of the analytic
+sphere: a ring of 8 sensors at radius 1 around it, alternately 0.3 above and below its equator, each casting
+lidar_directions(128, n_azimuth, (-37, 37)) with n_azimuth chosen for about --points returns (gt_geometry.scan_mesh,
+SPEC S22); the points then take the kNN normal preprocess with the sensor flip (64 neighbours, 85 degrees), as
+examples/recons_waymo.py does.  The setup line reports the scan's rays, returns and time.
 --out saves {'state_dict': ...}, which load_checkpoint_from_url(<path>) + load_state_dict take."""
 import argparse
 import json
@@ -80,9 +86,39 @@ def build_mesh_gt(W, device):
     return MeshGroundTruth(torch.from_numpy(v).to(device), torch.from_numpy(f).to(device), tau=2.0 * W)
 
 
-def make_scene(kind, n, depth, device, vol_sup=False, mesh_gt=False):
+SCAN_SENSORS, SCAN_BEAMS, SCAN_ELEVATION = 8, 128, (-37.0, 37.0)   # --mesh-scan: the sphere spans about +-20 degrees
+
+
+def scan_input(gt, n, device):
+    """the input of --mesh-scan: points of a simulated scan of gt's mesh after the kNN normal preprocess with the
+    sensor flip, their normals, and the scan's statistics"""
+    import math
+    import torch
+    from nksr_b200 import _lib
+    from nksr_b200.gt_geometry import lidar_directions, scan_mesh
+    from nksr_b200.reconstructor import estimate_normals_knn
+    a = 2.0 * math.pi * torch.arange(SCAN_SENSORS, dtype=torch.float64) / SCAN_SENSORS
+    z = 0.3 * (1.0 - 2.0 * (torch.arange(SCAN_SENSORS) % 2))
+    sensors = torch.stack([torch.cos(a), torch.sin(a), z], dim=1).float()
+    # about 4.5 % of the rays of each sensor meet the sphere
+    n_azimuth = max(64, int(round(n / (0.045 * SCAN_SENSORS * SCAN_BEAMS))))
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    scan = scan_mesh(gt.mesh, sensors, lidar_directions(SCAN_BEAMS, n_azimuth, SCAN_ELEVATION))
+    e1.record()
+    r = estimate_normals_knn(scan.xyz, scan.sensor, 64, 85.0)
+    s = _lib.exclusive_scan32(r.keep)
+    cnt = int(s[-1].item())
+    px, pn = (_lib.compact_rows(x, r.keep, s, cnt) for x in (r.xyz, r.normal))
+    torch.cuda.synchronize()
+    return px, pn, dict(rays=SCAN_SENSORS * SCAN_BEAMS * n_azimuth, returns=int(scan.xyz.shape[0]), kept=cnt,
+                        scan_ms=round(e0.elapsed_time(e1), 3))
+
+
+def make_scene(kind, n, depth, device, vol_sup=False, mesh_gt=False, mesh_scan=False):
     """the TrainingScene, and with vol_sup the volume's grid, build time (ms) and class fractions; with mesh_gt the
-    mesh's triangles and set-up time (ms, the icosphere's construction on the host included)"""
+    mesh's triangles and set-up time (ms, the icosphere's construction on the host included), and with mesh_scan
+    the scan's statistics"""
     import numpy as np
     import torch
     from nksr_b200.training import TrainingScene
@@ -98,9 +134,12 @@ def make_scene(kind, n, depth, device, vol_sup=False, mesh_gt=False):
         gt = build_mesh_gt(W, device)
         e1.record()
         torch.cuda.synchronize()
-        return (TrainingScene(t(xyz), t(nrm), W, depth, gt=gt),
-                dict(triangles=gt.mesh.n_tri, samples=int(gt.xyz.shape[0]), tau=gt.tau,
-                     setup_ms=round(e0.elapsed_time(e1), 3)))
+        info = dict(triangles=gt.mesh.n_tri, samples=int(gt.xyz.shape[0]), tau=gt.tau,
+                    setup_ms=round(e0.elapsed_time(e1), 3))
+        if not mesh_scan:
+            return TrainingScene(t(xyz), t(nrm), W, depth, gt=gt), info
+        px, pn, info["scan"] = scan_input(gt, n, device)
+        return TrainingScene(px, pn, W, depth, gt=gt), info
     px, pn, ps, W = cfg4_crop(n, device)
     if not vol_sup:
         return TrainingScene(px, pn, W, depth), None
@@ -231,6 +270,8 @@ def main(argv=None):
                     help="cfg4: volume ground truth from the sensor rays (DESIGN.md SPEC S19)")
     ap.add_argument("--mesh-gt", action="store_true",
                     help="sphere: mesh ground truth, an icosphere of the scene's radius (DESIGN.md SPEC S21)")
+    ap.add_argument("--mesh-scan", action="store_true",
+                    help="--mesh-gt: the input is a simulated LiDAR scan of the mesh (DESIGN.md SPEC S22)")
     ap.add_argument("--operator", choices=("assembled", "matrix_free"), default=None,
                     help="--kernel-losses: the kernel solve's operator (default: assembled)")
     ap.add_argument("--geometry", choices=("kernel", "neural"), default="kernel",
@@ -244,6 +285,8 @@ def main(argv=None):
         ap.error("--vol-sup needs --scene cfg4 (its points carry their sensor positions)")
     if args.mesh_gt and args.scene != "sphere":
         ap.error("--mesh-gt needs --scene sphere (its ground-truth mesh is the icosphere of the same radius)")
+    if args.mesh_scan and not args.mesh_gt:
+        ap.error("--mesh-scan needs --mesh-gt (it scans the ground-truth mesh)")
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("train_unet.py needs a CUDA device")
@@ -254,7 +297,7 @@ def main(argv=None):
     from nksr_b200.network import NKSRNetwork
     torch.use_deterministic_algorithms(True, warn_only=True)
     dev = torch.device("cuda:0")
-    scene, vol = make_scene(args.scene, args.points, args.depth, dev, args.vol_sup, args.mesh_gt)
+    scene, vol = make_scene(args.scene, args.points, args.depth, dev, args.vol_sup, args.mesh_gt, args.mesh_scan)
     net = NKSRNetwork(dict(backbone="unet", tree_depth=args.depth, kernel_dim=4, precision=args.precision,
                            trainable=True, seed=args.seed, structure=args.structure,
                            udf=dict(enabled=args.udf), geometry=args.geometry)).to(dev)
